@@ -11,7 +11,7 @@ batch 64 per GPU, synthetic data, random-init weights.
 Prints ONE JSON line (rank 0).  value = whole-job images/sec with inputs resident in HBM;
 e2e = same step driven through the public API from pinned HOST buffers (H2D of the batch and D2H of the loss
 inside the timed region).  Extra objects: roofline (dominant kernel) + layers (top launches against their own roofline),
-cpu_baseline (the reference on the host cores), gpu_baseline (the reference's modules as stock PyTorch on the same B200),
+cpu_baseline (the reference on the host cores), gpu_baseline (the reference's modules as stock PyTorch on the same GPU),
 parity (logit error / label mismatch of every execution mode against the fp32 CUDA-core executor), modes (step time of the
 fp16 and fp16x3 modes).
 """
@@ -53,8 +53,10 @@ def parse():
     ap.add_argument("--cpu-sample", type=int, default=8, help="images per CPU-baseline step")
     ap.add_argument("--skip-cpu", action="store_true", help="profiling runs: skip the CPU baseline leg")
     ap.add_argument("--skip-e2e", action="store_true", help="profiling runs: skip the host-buffer leg")
-    ap.add_argument("--skip-gpu-baseline", action="store_true", help="skip the stock-PyTorch-on-B200 leg")
+    ap.add_argument("--skip-gpu-baseline", action="store_true", help="skip the stock-PyTorch-on-the-same-GPU leg")
     ap.add_argument("--skip-extras", action="store_true", help="skip parity / other-mode timing")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's loss and outputs to DIR/<name>.npy (float32), and the per-launch kernel table to DIR/kernel_detail.txt")
     return ap.parse_args()
 
 
@@ -63,7 +65,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d["bf16_tflops_sustained"], "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "src": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- upper bounds, not measured rates
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 def host_cores():
@@ -101,7 +104,7 @@ def synth(n, seed):
 
 
 # ----------------------------------------------------------------------------------------------
-# The reference itself (unmodified modules staged by oracle/build_ref.py): CPU arm and stock-PyTorch-on-B200 arm.
+# The reference itself (unmodified modules staged by oracle/build_ref.py): CPU arm and stock-PyTorch-on-the-same-GPU arm.
 # The only places bench.py touches oracle/.
 # ----------------------------------------------------------------------------------------------
 _REF = {}
@@ -212,7 +215,7 @@ def run_reference(args):
 
 
 def gpu_reference_baseline(args, dev, img_d, lab_d):
-    """The reference's modules as stock PyTorch (ATen / cuDNN) on the same B200: the kernel to beat (SURVEY F1, 8(d))."""
+    """The reference's modules as stock PyTorch (ATen / cuDNN) on the same GPU: the kernel to beat (SURVEY F1, 8(d))."""
     mods = load_reference()
     if mods is None:
         return {"unavailable": "reference files not staged (oracle/_ref/reference_code.tar missing)"}
@@ -372,6 +375,27 @@ def time_other_modes(args, dev, img_d, lab_d, world):
     return out
 
 
+DUMP_MAX_ELEMS = 1 << 22        # per array: 16 MB of float32; larger outputs are sampled at fixed, seeded positions
+
+
+def dump_outputs(out_dir, loss, step):
+    """What the timed path handed back in its last step (the loss, and the logits of each head where the step keeps them),
+    as float32 .npy files.  Inputs and weights are seeded, so two builds run with the same arguments can be compared
+    file by file."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss.detach().float().reshape(1)}
+    for i, o in enumerate(getattr(step, "outputs", None) or []):
+        if torch.is_tensor(o):
+            arrays[f"output{i}"] = o.detach().float()
+    for name, t in arrays.items():
+        if t.numel() > DUMP_MAX_ELEMS:
+            idx = torch.randperm(t.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_MAX_ELEMS].sort().values
+            t = t.reshape(-1)[idx.to(t.device)]
+            name += "_sample"
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
+
+
 def main():
     args = parse()
     if args.impl == "reference":
@@ -457,6 +481,8 @@ def main():
     barrier()
     ms_dev = ev0.elapsed_time(ev1)
     launches_eager = _lib.COUNTERS["launch_calls"] - c0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, step)
 
     # ---- timed region 2: end to end from pinned host memory, loss read back every step ----
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -537,11 +563,12 @@ def main():
                 d["bytes"] += meta[3] * cnt
         detail = sorted(((name, meta[0], meta[1], cnt, ms / cnt, meta[2] / (ms / cnt * 1e-3) / 1e12, meta[3] / (ms / cnt * 1e-3) / 1e9, meta[2], meta[3])
                          for (name, meta), (cnt, ms) in agg.items() if meta is not None), key=lambda r: -r[3] * r[4])
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        with open(os.path.join(ROOT, "gpurun_out", "kernel_detail.txt"), "w") as f:
-            f.write("entry kind layer launches avg_ms TFLOP/s algorithmic_GB/s\n")
-            for r in detail:
-                f.write(f"{r[0]} {r[1]} {r[2]} {r[3] // n_prof} {r[4]:.4f} {r[5]:.1f} {r[6]:.0f}\n")
+        if args.dump_outputs:                        # the tree itself may be read-only: per-launch detail goes with the dumps
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            with open(os.path.join(args.dump_outputs, "kernel_detail.txt"), "w") as f:
+                f.write("entry kind layer launches avg_ms TFLOP/s algorithmic_GB/s\n")
+                for r in detail:
+                    f.write(f"{r[0]} {r[1]} {r[2]} {r[3] // n_prof} {r[4]:.4f} {r[5]:.1f} {r[6]:.0f}\n")
         # top launches, each against the roofline that bounds it (per-kernel event timing: burst tensor peak, measured copy GB/s)
         ridge = peaks["tf_burst"] * 1e12 / (peaks["hbm_gbs"] * 1e9)
         layers = []
@@ -561,25 +588,17 @@ def main():
                  for k, v in sorted(byname.items(), key=lambda kv: -kv[1]["ms"])}
         top = max(byname.items(), key=lambda kv: kv[1]["ms"])
         name, v = top
-        traffic = None
-        for tp in ("r2_traffic.json", "r1_traffic.json"):
-            tpath = os.path.join(ROOT, "profiles", tp)
-            if os.path.exists(tpath):
-                tj = json.load(open(tpath))
-                if tj.get("kernel") == name:
-                    traffic = {"dram_MB_per_launch": round(tj["dram_bytes_per_launch_MB"], 1), "source": tj["source"]}
-                    break
         if v["flops"] > 0:
             ach = v["flops"] / (v["ms"] * 1e-3) / 1e12
             roof = {"kernel": name, "bound": "tensor", "achieved": round(ach, 2), "peak": peaks["tf_burst"], "unit": "TFLOP/s",
-                    "frac": round(ach / peaks["tf_burst"], 4), "frac_of_sustained": round(ach / peaks["tf_sustained"], 4), "traffic": traffic,
+                    "frac": round(ach / peaks["tf_burst"], 4), "frac_of_sustained": round(ach / peaks["tf_sustained"], 4),
                     "algorithmic_MB_per_launch": round(v["bytes"] / v["launches"] / 1e6, 1),
                     "peak_source": peaks["src"] + " bf16 burst (kernels timed one by one with CUDA events; the step is not power-limited)",
                     "avg_launch_ms": round(v["ms"] / v["launches"], 4), "algorithmic_flops_per_launch": v["flops"] / v["launches"]}
         else:
             ach = v["bytes"] / (v["ms"] * 1e-3) / 1e9 if v["bytes"] else 0.0
             roof = {"kernel": name, "bound": "hbm", "achieved": round(ach, 1), "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                    "frac": round(ach / peaks["hbm_gbs"], 4), "traffic": traffic, "peak_source": peaks["src"],
+                    "frac": round(ach / peaks["hbm_gbs"], 4), "peak_source": peaks["src"],
                     "avg_launch_ms": round(v["ms"] / v["launches"], 4), "algorithmic_MB_per_launch": round(v["bytes"] / v["launches"] / 1e6, 1)}
 
     lps, graph_on = step.launches_per_step, getattr(step, "captured", step.graph_enabled)   # launches per step counted at capture time
@@ -605,7 +624,7 @@ def main():
                        "precision": args.precision, "cuda_graph": bool(graph_on),
                        "comm": getattr(step, "comm_mode", None) if world > 1 else None,
                        "bn": "per-rank batch statistics (stock DDP semantics)",
-                       "l2": "per-step working set (~6 GB of activations) >> 126 MB L2; no explicit flush needed"},
+                       "l2": "per-step working set (~6 GB of activations) >> 50 MB L2; no explicit flush needed"},
             "e2e": {"value": imgs / (ms_e2e * 1e-3), "unit": "images/sec", "ms_per_step": ms_e2e / K,
                     "h2d_bytes_per_step": int(img_h.numel() * 4 + lab_h.numel()), "d2h_bytes_per_step": 4},
             "gpu_launches": (lps * K) if graph_on else launches_eager,

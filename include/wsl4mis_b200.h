@@ -1,5 +1,5 @@
 /*
- * wsl4mis_b200 -- C ABI of the B200 (sm_100a) kernels behind the WSL4MIS segmentation-training hot path.
+ * wsl4mis_b200 -- C ABI of the H100 (sm_90a) kernels behind the WSL4MIS segmentation-training hot path.
  *
  * The reference (HiLab-git/WSL4MIS) has no native code and no FFI: every operation below is, in the reference,
  * a stock PyTorch call made from Python.  Each entry point therefore cites the reference *Python* call site
@@ -13,7 +13,7 @@
  *   - return 0 on success, negative on error; wsl_last_error() returns a thread-local message;
  *   - "act" tensors are channels-last (NHWC); their storage type is bf16 (`dtype` 0, the fast tensor-core path),
  *     fp32 (`dtype` 1: the reference-accurate parity modes -- CUDA-core direct convolutions, or the fp16 hi/lo split
- *     tensor-core convolutions wsl_conv_tc_split / wsl_wgrad_tc_split) or fp16 (`dtype` 2: same tcgen05 kind::f16 rate as
+ *     tensor-core convolutions wsl_conv_tc_split / wsl_wgrad_tc_split) or fp16 (`dtype` 2: same wgmma rate as
  *     bf16 with an 11-bit mantissa; gradients then travel multiplied by a power-of-two loss scale chosen by the caller);
  *     logits / probabilities / losses are fp32 NCHW;
  *   - `ws` is a caller-provided workspace of wsl_workspace_floats() floats, zero-initialised ONCE by the
@@ -157,7 +157,7 @@ int wsl_conv_first(const float* x, const float* w, const float* bias, void* y, i
 int wsl_wgrad_first(const float* x, const void* dy, int dtype, float* dw, int N, int H, int W, int Cout,
                     cudaStream_t stream);
 
-/* tcgen05 implicit-GEMM convolution (conv_tc.cu): same contract as wsl_conv_direct for 16-bit NHWC sources (dtype 0 = bf16,
+/* wgmma implicit-GEMM convolution (conv_tc.cu): same contract as wsl_conv_direct for 16-bit NHWC sources (dtype 0 = bf16,
  * 2 = fp16: operands, packed weights and out_mode-0 outputs all have that type) with channel counts that are multiples
  * of 16.  wpk_bf16: [taps][CoutP][CinP] (K-major).  Requires wsl_tc_available(). */
 int wsl_tc_available(void);
@@ -165,7 +165,7 @@ int wsl_conv_tc(const void* src0, int C0, const void* src1, int C1, const void* 
                 void* out, int out_mode, int N, int H, int W, int CoutP, int CoutStore, int ksize, int dtype,
                 cudaStream_t stream);
 /* v2 of the same convolution: persistent CTAs, weights resident in shared memory, one halo load per pixel tile whose
- * nine taps are row-shifted UMMA descriptor views (no reload).  Same contract; needs W % 8 == 0 and H % 16 == 0. */
+ * nine taps are row-shifted wgmma descriptor views (no reload).  Same contract; needs W % 8 == 0 and H % 16 == 0. */
 int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, const void* wpk_bf16, const float* bias,
                  void* out, int out_mode, int N, int H, int W, int CoutP, int CoutStore, int ksize, int dtype,
                  float* stat_partials, int* stat_rows_host, cudaStream_t stream);
@@ -175,7 +175,7 @@ int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, const void*
 int wsl_bn_finalize(const float* partials, int nrows, long long P, int C, const float* gamma, const float* beta,
                     float* running_mean, float* running_var, long long* num_batches_tracked, float momentum, float eps,
                     float* save, float* ss, cudaStream_t stream);
-/* tcgen05 weight gradient (conv_tc.cu): dw (fp32, torch layout [CoutReal][C0+C1][k][k]) += dY^T * X over all pixels.
+/* wgmma weight gradient (conv_tc.cu): dw (fp32, torch layout [CoutReal][C0+C1][k][k]) += dY^T * X over all pixels.
  * Bias gradients are NOT produced here (see wsl_channel_sum). */
 int wsl_wgrad_tc(const void* src0, int C0, const void* src1, int C1, const void* dy, int CoutP, float* dw, int N, int H,
                  int W, int CoutReal, int ksize, int dtype, float* partial_ws, long long partial_floats, cudaStream_t stream);
@@ -206,7 +206,7 @@ int wsl_wgrad_tc_split(const void* x_staged, int Cin, const float* x_inv_scale, 
                        const float* dy_inv_scale, float* dw, int N, int H, int W, int CoutReal, int ksize, int dilation,
                        cudaStream_t stream);
 
-/* dilated 3x3 convolution of PNet2D's blocks (networks/pnet.py:25-28, dilation = padding = 1, 2, 4, 8, 16) on the per-tap tcgen05
+/* dilated 3x3 convolution of PNet2D's blocks (networks/pnet.py:25-28, dilation = padding = 1, 2, 4, 8, 16) on the per-tap wgmma
  * kernel: tap (dy, dx) is the TMA box at (y0 + dilation*dy, x0 + dilation*dx), out-of-bounds zero fill = the padding; with the flipped /
  * transposed pack it is the data gradient; wsl_wgrad_tc_dil is the matching weight gradient.  LeakyReLU backward without BatchNorm for the
  * 1x1 heads (pnet.py:54-59,75-81). */

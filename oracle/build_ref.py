@@ -7,7 +7,7 @@ output, like the compiled .so: it stays out of history but travels to the GPU bo
 The reference is pure Python: "building" it is copying the files where they lie.  Nothing here is edited, and nothing
 under wsl4mis_b200/ or dropin/ may import from oracle/_ref (tests/test_abi_cpu.py checks).  Users of the staged files:
   * bench.py --impl reference     the reference's own modules on the host CPU (cpu_baseline kind "reference")
-  * bench.py gpu_baseline         the same modules on cuda: stock PyTorch on the same B200, the real kernel to beat
+  * bench.py gpu_baseline         the same modules on cuda: stock PyTorch on the same GPU, the real kernel to beat
   * tests/test_gpu_scripts.py     runs the reference's train_*.py scripts UNCHANGED on top of dropin/ (SURVEY 8(b))
 """
 import hashlib

@@ -129,7 +129,7 @@ def _q(x):
 
 
 def _qw(w, x):
-    """weights are 16-bit on the tcgen05 path: Cin % 16 == 0 and the map is a multiple of the 8x16 pixel tile"""
+    """weights are 16-bit on the wgmma path: Cin % 16 == 0 and the map is a multiple of the 8x16 pixel tile"""
     if QUANT is None:
         return w
     tc = (w.shape[1] % 16 == 0) and (x.shape[-1] % 16 == 0) and (x.shape[-2] % 8 == 0)

@@ -1,4 +1,4 @@
-"""Diagnostic (not collected by pytest): the reference step as STOCK EAGER PYTORCH ON THE SAME B200 -- SURVEY 8(d)'s "real
+"""Diagnostic (not collected by pytest): the reference step as STOCK EAGER PYTORCH ON THE SAME GPU -- SURVEY 8(d)'s "real
 kernel to beat" (the reference is a plain PyTorch program; /root/reference does not exist on the GPU box, so its pinned
 functional restatement oracle/wsl_oracle.py is run on cuda tensors: same ATen/cuDNN operators, GatedCRF in the reference's
 materialising F.unfold formulation).  Batch 16 bounds the unfold temporaries (~12 GB with autograd); images/s is reported

@@ -79,7 +79,7 @@ def test_ramps():
 
 
 def test_dropin_shim_exposes_the_reference_module_names():
-    """`dropin/` ahead of the reference's code/ on PYTHONPATH gives the scripts' own import lines the B200 modules
+    """`dropin/` ahead of the reference's code/ on PYTHONPATH gives the scripts' own import lines the H100 modules
     (train_weakly_supervised_pCE_GatedCRFLoss_2D.py:23-28)."""
     import importlib
     import sys

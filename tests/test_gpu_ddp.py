@@ -1,4 +1,4 @@
-"""Data-parallel step on two real GPUs (NCCL): run with `gpurun --gpus 2 -- python -m pytest tests/test_gpu_ddp.py -m gpu`.
+"""Data-parallel step on two real GPUs (NCCL): run with `python -m pytest tests/test_gpu_ddp.py -m gpu` on a machine with two GPUs.
 Skipped on a single-GPU box.
 
   * replicas stay BIT-identical over several steps (every rank applies the same all-reduced bucket to the same weights);
@@ -77,7 +77,7 @@ def _worker(rank, world, port, variant, graph, out):
 def _run(variant, graph):
     import torch.multiprocessing as mp
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs (gpurun --gpus 2)")
+        pytest.skip("needs two GPUs")
     mgr = mp.Manager()
     out = mgr.dict()
     mp.spawn(_worker, args=(2, _free_port(), variant, graph, out), nprocs=2, join=True)
@@ -163,7 +163,7 @@ def test_global_batch_mode_equals_the_single_process_step(variant):
     import random
     import torch.multiprocessing as mp
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs (gpurun --gpus 2)")
+        pytest.skip("needs two GPUs")
     mgr = mp.Manager()
     out = mgr.dict()
     mp.spawn(_worker_global, args=(2, _free_port(), variant, out), nprocs=2, join=True)

@@ -142,8 +142,7 @@ def test_uamt_step_matches_oracle(precision):
 def _lockstep(eager, captured, calls, state):
     """Step an eager and a graph-captured stepper side by side on the same inputs and compare EVERY step's loss and weights, then
     copy the eager state over the captured one.  (The fp32 cross-check mode accumulates weight gradients with atomics; run to run
-    that is 1e-8 of noise which training amplifies ~4x per step -- measured on the B200: identical losses for two steps, 2e-4 apart
-    after ten -- so a comparison of final weights after many free-running steps cannot tell a stale ramp from noise.  One step from
+    that is 1e-8 of noise which training amplifies ~4x per step, so a comparison of final weights after many free-running steps cannot tell a stale ramp from noise.  One step from
     identical state can: noise stays ~1e-9, a wrong EMA factor or ramp value is >= 1e-4.)"""
     worst = 0.0
     for i, call_args in enumerate(calls):

@@ -191,7 +191,7 @@ WGRAD_TC_CASES += [(2, 32, 32, 16, 0, 16, 3), (1, 64, 32, 32, 32, 32, 3), (2, 32
 @pytest.mark.parametrize("case", WGRAD_TC_CASES)
 @pytest.mark.parametrize("ver", ["wsl_wgrad_tc", "wsl_wgrad_tc2", "wsl_wgrad_tc3", "wsl_wgrad_tc3-fp16"])
 def test_wgrad_tc(case, ver):
-    """tcgen05 weight gradient vs fp64 autograd on the same 16-bit inputs; fp32 accumulation -> 1e-4 relative."""
+    """wgmma weight gradient vs fp64 autograd on the same 16-bit inputs; fp32 accumulation -> 1e-4 relative."""
     N, H, W, C0, C1, Cout, ks = case
     dt = 2 if ver.endswith("-fp16") else 0
     ver = ver.split("-")[0]
@@ -554,7 +554,7 @@ def test_channel_sum_any_width(dt, C, Creal, det):
 @pytest.mark.parametrize("dil", [2, 4, 16])
 @pytest.mark.parametrize("dt", [0, 2])
 def test_dilated_convolution(dil, dt):
-    """PNet2D's dilated 3x3 blocks (networks/pnet.py:25-28) on the per-tap tcgen05 kernel: forward, data gradient and weight gradient
+    """PNet2D's dilated 3x3 blocks (networks/pnet.py:25-28) on the per-tap wgmma kernel: forward, data gradient and weight gradient
     against fp64 F.conv2d(dilation=d, padding=d) on the same 16-bit inputs."""
     N, H, W, C, Cout, ks = 2, 32, 32, 64, 64, 3
     g = torch.Generator().manual_seed(100 + dil)

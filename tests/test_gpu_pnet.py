@@ -1,5 +1,5 @@
 """PNet2D (SURVEY 8(f) rank 4; reference networks/pnet.py, net_factory.py:18-19) on the planned executor: dilated 3x3 blocks on the per-tap
-tcgen05 kernel, concat + 1x1 heads, Dropout2d -- against the fixture generated from the unmodified reference class."""
+wgmma kernel, concat + 1x1 heads, Dropout2d -- against the fixture generated from the unmodified reference class."""
 import os
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""The reference's OWN training scripts, unchanged, on the B200 modules (SURVEY 8(b); VERDICT r1 item 5).
+"""The reference's OWN training scripts, unchanged, on the H100 modules (SURVEY 8(b); VERDICT r1 item 5).
 
 The unmodified `train_*.py` files come from the archive `oracle/build_ref.py` staged in the build container (git-ignored, it
 travels with the tree; /root/reference does not exist on the GPU box).  Each test unpacks it into a scratch `code/` directory,

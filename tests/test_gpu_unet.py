@@ -377,7 +377,7 @@ def test_unet_ds_bf16_path_matches_the_quant_oracle(golden_dir):
 
 
 def test_unet_ds_wide_input_runs_the_tensor_core_heads():
-    """64 x 128 input: the dp1 / dp2 heads take the tcgen05 kernels; outputs against the bf16-emulating oracle, backward runs."""
+    """64 x 128 input: the dp1 / dp2 heads take the wgmma kernels; outputs against the bf16-emulating oracle, backward runs."""
     from wsl4mis_b200.networks.unet import UNet_DS
     N, H, W = 2, 64, 128
     p = O.synth_params(1, 4, ("decoder",), 41, ds=True)

@@ -1,4 +1,4 @@
-"""wsl4mis_b200 -- B200-native (sm_100a) kernels for the WSL4MIS segmentation-training hot path.
+"""wsl4mis_b200 -- H100-native (sm_90a) kernels for the WSL4MIS segmentation-training hot path.
 
 Public surface mirrors the reference's ``code/networks`` and ``code/utils`` modules:
     wsl4mis_b200.networks.unet / net_factory

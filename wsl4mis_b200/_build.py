@@ -1,4 +1,4 @@
-"""Build the C-ABI CUDA library in-tree with nvcc (sm_100a only).
+"""Build the C-ABI CUDA library in-tree with nvcc (sm_90a only).
 
     python -m wsl4mis_b200._build        # or __graft_entry__.build()
 
@@ -14,7 +14,7 @@ CSRC = os.path.join(PKG, "csrc")
 OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(PKG, "libwsl4mis_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--use_fast_math=false"]
 FLAGS = [f for f in FLAGS if not f.startswith("--use_fast_math")]
 

@@ -1,4 +1,4 @@
-// Shared helpers for the wsl4mis_b200 C-ABI library (sm_100a only).
+// Shared helpers for the wsl4mis_b200 C-ABI library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -17,6 +17,18 @@ int  wsl_check_launch(const char* what);
     if (!(cond)) { wsl_set_error(__VA_ARGS__); return -1; }     \
   } while (0)
 
+// SMs of the current device (132 on an H100 SXM, 114 on an H100 PCIe, fewer on a MIG slice): grids are sized in waves of
+// resident CTAs over them.  Queried once per device.
+inline int wsl_num_sms() {
+  static int cache[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (cache[dev] == 0) {
+    int n = 0;
+    cache[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
+  }
+  return cache[dev];
+}
 constexpr int WSL_MAX_PARTIAL_BLOCKS = 2048;   // every reduction kernel launches <= this many CTAs
 constexpr int WSL_WS_FLOATS = 1 << 20;  // per-call workspace (floats, 4 MiB), zero-initialised once; [0,64) tickets, rest partials
 

@@ -1,20 +1,22 @@
-// tcgen05 implicit-GEMM convolution for sm_100a (3x3 pad 1 / 1x1) on channels-last bf16 activations.
+// wgmma implicit-GEMM convolution for sm_90a (3x3 pad 1 / 1x1) on channels-last bf16 activations.
 //
-//   D[128 pixels, NT couts] (fp32, TMEM) = sum_{tap} sum_{kblock} A_tap[128 x KBLK] * B_tap[KBLK x NT]
+//   D[128 pixels, NT couts] (fp32, registers) = sum_{tap} sum_{kblock} A_tap[128 x KBLK] * B_tap[KBLK x NT]
 //
 //   * A: one TMA 4-D box (KBLK channels x 16 w x 8 h x 1 image) per (tap, k-block) at the tap-shifted pixel
 //     coordinate; TMA's out-of-bounds zero fill IS the convolution's zero padding (im2col-free).
 //   * B: packed weights [tap][Cout][Cin] bf16 (K-major), one 3-D box (KBLK x NT x 1) per (tap, k-block).
 //   * both land in 128B/64B/32B-swizzled shared memory (swizzle span = KBLK*2 bytes) and are consumed by
-//     tcgen05.mma.cta_group::1.kind::f16 (M=128, N=NT, K=16) issued by one elected thread; fp32 accumulators in TMEM.
-//   * warp roles: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM alloc), warps 2..5 = epilogue
-//     (tcgen05.ld 32x32b -> +bias -> bf16 NHWC / fp32 NCHW stores).
-//   * mbarrier ring (full/empty) of STAGES stages between TMA and MMA; tcgen05.commit releases a stage.
+//     wgmma.mma_async (M = 64, N = NT, K = 16) straight from shared memory; fp32 accumulators in registers.
+//   * thread roles (every kernel in this file): warpgroups 0 and 1 = consumers, each owning accumulator rows
+//     64*h .. 64*h+63 of the 128-row tile (MMA issue + epilogue from its registers); warpgroup 2 = producer (warp 8 issues TMA).
+//   * mbarrier ring (full/empty) of STAGES stages between TMA and the consumers; every consumer warp releases a stage
+//     once its wgmma group has retired.
 //
 // The same kernel is the data-gradient (dgrad) kernel when fed tap-flipped, transposed weights, and the 1x1
 // convolution with TAPS = 1.  Two source tensors model torch.cat([skip, up], 1) without materialising it.
 // Reference call sites: networks/unet.py:19,23 (3x3), :55 (1x1), :67 (concat), :120 (out_conv).
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <mutex>
 #include <unordered_map>
@@ -46,18 +48,16 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must abort the kernel (trap -> launch error), never hang the GPU.
+// Bounded wait: a protocol bug must abort the kernel (trap -> launch error), never hang the GPU.  No printf here: any
+// function call inside a wgmma kernel makes ptxas serialise every wgmma.mma_async of that kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  for (uint32_t spin = 0; !mbar_try_wait(bar, parity); ++spin) {
-    if (spin > (1u << 24)) {
-      printf("wsl conv_tc: mbarrier timeout (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y, threadIdx.x);
-      __trap();
-    }
-  }
+  for (uint32_t spin = 0; !mbar_try_wait(bar, parity); ++spin)
+    if (spin > (1u << 24)) __trap();
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
   asm volatile(
@@ -74,100 +74,58 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* ba
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
 }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// Issue-path helpers.  The MMA warp stays converged; ONE elected lane issues, and every operand of the issue loop is a
-// warp-uniform value (read through lane 0), so the compiler keeps descriptors in uniform registers and emits back-to-back
-// UTCHMMA instead of a per-instruction ELECT / R2UR / branch sequence (measured on the B200: ~80 -> ~50 cycles per
-// M=128,N=16 MMA; profiles/micro/mma_rate.cu).  A descriptor is {lo = addr>>4 | LBO<<16, hi = constant}.
 __device__ __forceinline__ uint32_t elect_one() {
   uint32_t e;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(e));
   return e;
 }
 __device__ __forceinline__ uint32_t uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
-__device__ __forceinline__ void umma_f16_w(uint32_t tmem_d, uint32_t alo, uint32_t ahi, uint32_t blo, uint32_t bhi, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(alo), "r"(ahi), "r"(blo), "r"(bhi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// high word of a shared-memory descriptor: SBO | version 1 | swizzle layout
+
+// wgmma shared-memory descriptor of a swizzled operand (swizzle span SW = 32/64/128 bytes, the TMA box's swizzle):
+//   K-major:  8-row groups SBO bytes apart (LBO unused);
+//   MN-major: SW-byte wide groups along M/N LBO bytes apart, 8-row groups along K SBO bytes apart.
+// Several kernels view one TMA tile through descriptors whose start is shifted by whole rows (the taps of a 3x3 halo):
+// the tensor core takes the swizzle phase from the absolute shared-memory address, as TMA does, so base_offset stays 0.
 template <int SW>
-__host__ __device__ constexpr uint32_t desc_hi(uint32_t sbo_bytes) {
-  return ((sbo_bytes >> 4) & 0x3fffu) | (1u << 14) | (((SW == 128) ? 2u : (SW == 64) ? 4u : 6u) << 29);
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  constexpr uint64_t layout = (SW == 128) ? 1 : (SW == 64) ? 2 : 3;
+  return (uint64_t)((saddr & 0x3ffff) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32) | (layout << 62);
 }
 
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+// Fragment coordinates of a consumer thread (t = thread index inside its warpgroup): accumulator element
+// acc[4*j + 2*i + b] is row frag_row(t) + 8*i of the warpgroup's 64 rows, column 8*j + frag_col(t) + b.
+__device__ __forceinline__ int frag_row(int t) { return 16 * (t >> 5) + ((t & 31) >> 2); }
+__device__ __forceinline__ int frag_col(int t) { return 2 * (t & 3); }
+
+// Two consumer warpgroups and one producer warpgroup (only its first warp issues TMA).  Registers are allocated per warpgroup, so
+// the producer warpgroup hands its share to the consumers: 40 + 2 x 232 registers per thread-slot of a warpgroup fill the file.
+constexpr int CONSUMER_WARPS = 8, CONSUMERS = 32 * CONSUMER_WARPS, NUM_THREADS = CONSUMERS + 128, PRODUCER_WARP = CONSUMER_WARPS;
+__device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory"); }
+__device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory"); }
+// consumer warp retired its wgmma group: one arrival per warp (empty barriers count CONSUMER_WARPS)
+__device__ __forceinline__ void release_stage(uint64_t* bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory descriptor, K-major operand, swizzle span = SW bytes (32/64/128):
-//   canonical layout ((8,m),(T,2)):((SW/16,SBO),(1,.)) in 16-byte units -> 8-row groups SBO = 8*SW bytes apart.
-template <int SW>
-__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t saddr) {
-  constexpr uint64_t layout = (SW == 128) ? 2 : (SW == 64) ? 4 : 6;
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3ffff) >> 4);          // start address  [0,14)
-  d |= (uint64_t)1 << 16;                            // LBO (ignored for swizzled K-major) [16,30)
-  d |= (uint64_t)((8 * SW) >> 4) << 32;              // SBO [32,46)
-  d |= (uint64_t)1 << 46;                            // descriptor version (Blackwell)
-  d |= layout << 61;                                 // swizzle mode
-  return d;
-}
-
-// instruction descriptor: D=f32, A=B=bf16, both K-major, M=128, N=n
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int n, int a_mn_major = 0, int b_mn_major = 0, int m = 128) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-// the same descriptor for the run-time 16-bit operand type: dt 0 = bf16 (format code 1), dt 2 = fp16 (format code 0);
-// kind::f16 runs both at the same rate, fp16 carries an 11-bit instead of an 8-bit mantissa
-__device__ __forceinline__ uint32_t idesc_for(uint32_t idesc_bf16, int dt) {
-  return dt == 2 ? (idesc_bf16 & ~((1u << 7) | (1u << 10))) : idesc_bf16;
+// Stores two adjacent output channels (c, c + 1) of one pixel.  out_mode 0: 16-bit NHWC, 1: fp32 NCHW, 2: fp32 NHWC.
+__device__ __forceinline__ void store_pair(void* out, int out_mode, int dt, int CoutStore, int H, int W, int n, int gy, int gx,
+                                           int c, float v0, float v1) {
+  if (out_mode == 0) {
+    if (c < CoutStore) {
+      uint32_t* o = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(out) + (((long long)n * H + gy) * W + gx) * CoutStore + c);
+      *o = dt == 2 ? pack_f16(v0, v1) : pack_bf16(v0, v1);
+    }
+  } else if (out_mode == 2) {
+    float* o = reinterpret_cast<float*>(out) + (((long long)n * H + gy) * W + gx) * CoutStore + c;
+    if (c + 1 < CoutStore) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+    else if (c < CoutStore) o[0] = v0;
+  } else {
+    float* o = reinterpret_cast<float*>(out);
+    if (c < CoutStore) o[(((long long)n * CoutStore + c) * H + gy) * W + gx] = v0;
+    if (c + 1 < CoutStore) o[(((long long)n * CoutStore + c + 1) * H + gy) * W + gx] = v1;
+  }
 }
 
 struct ConvTcParams {
@@ -186,7 +144,6 @@ struct ConvTcParams {
 };
 
 constexpr int TILE_W = 16, TILE_H = 8, TILE_M = 128;
-constexpr int NUM_THREADS = 192;
 
 template <int KBLK, int NT, int STAGES>
 struct ConvSmem {
@@ -202,13 +159,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
                                                                  const __grid_constant__ CUtensorMap map_b, const ConvTcParams p) {
   using S = ConvSmem<KBLK, NT, STAGES>;
   constexpr int SW = KBLK * 2;
-  constexpr uint32_t TMEM_COLS = NT < 32 ? 32 : NT;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x;
@@ -221,20 +175,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
   const int iters = p.taps * (kb0 + kb1);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_WARPS); }
     fence_barrier_init();
     prefetch_tmap(&map_a0);
     prefetch_tmap(&map_b);
     if (kb1) prefetch_tmap(&map_a1);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= PRODUCER_WARP) {
+    producer_regs();
+    if (warp != PRODUCER_WARP) return;
     // ===================== TMA producer =====================
     if (lane == 0) {
       int it = 0;
@@ -253,78 +204,45 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = idesc_for(make_idesc_bf16(NT), p.dt);
-    for (int it = 0; it < iters; ++it) {
-      const int s = it % STAGES;
-      const uint32_t ph = (it / STAGES) & 1;
-      mbar_wait(&full_bar[s], ph);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES);
-        const uint32_t b_addr = a_addr + S::A_BYTES;
-        const uint64_t adesc = make_kmajor_desc<SW>(a_addr);
-        const uint64_t bdesc = make_kmajor_desc<SW>(b_addr);
+    return;
+  }
+  consumer_regs();
+  // ===================== consumers: warpgroup h owns pixel rows 64h .. 64h+63 =====================
+  const int h = threadIdx.x >> 7, t = threadIdx.x & 127;
+  float acc[NT / 2];
 #pragma unroll
-        for (int k = 0; k < KBLK / 16; ++k) {
-          // advance 16 elements (32 bytes) along K inside the swizzle span: +2 in the 16-byte start-address field
-          umma_f16(tmem_base, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[s]);                 // frees the smem stage when these MMAs retire
-        if (it == iters - 1) umma_commit(accum_bar); // accumulator complete -> epilogue
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int m = q * 32 + lane;            // accumulator row = pixel index inside the tile
+  for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+  for (int it = 0; it < iters; ++it) {
+    const int s = it % STAGES;
+    mbar_wait(&full_bar[s], (it / STAGES) & 1);
+    const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES) + (uint32_t)(h * 64 * SW);
+    const uint32_t b_addr = smem_u32(smem + s * S::STAGE_BYTES + S::A_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KBLK / 16; ++k)   // 16 elements (32 bytes) along K inside the swizzle span
+      Wgmma<NT>::template mma<0, 0>(acc, gmma_desc<SW>(a_addr + 32 * k, 16, 8 * SW), gmma_desc<SW>(b_addr + 32 * k, 16, 8 * SW),
+                                    (it > 0 || k > 0) ? 1u : 0u, p.dt);
+    wgmma_commit();
+    wgmma_wait<0>();
+    release_stage(&empty_bar[s]);
+  }
+  wgmma_fence_regs(acc);
+  // ===================== epilogue from registers =====================
+  const float sc = p.out_scale ? *p.out_scale : 1.f;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int m = 64 * h + frag_row(t) + 8 * i;   // pixel index inside the tile
     const int gy = y0 + m / TILE_W, gx = x0 + m % TILE_W;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const bool inb = (gy < p.H) && (gx < p.W);
-#pragma unroll 1
-    for (int c = 0; c < NT; c += 16) {
-      float v[16];
-      tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-      if (p.out_scale) {
-        const float sc = *p.out_scale;
+    if (gy >= p.H || gx >= p.W) continue;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] *= sc;
-      }
-      if (p.bias) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] += p.bias[n0 + c + j];
-      }
-      if (!inb) continue;
-      if (p.out_mode == 0) {
-        if (n0 + c < p.CoutStore) {
-          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + (((long long)n * p.H + gy) * p.W + gx) * p.CoutStore + n0 + c;
-          float lo[8], hi[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { lo[j] = v[j]; hi[j] = v[8 + j]; }
-          reinterpret_cast<uint4*>(o)[0] = pack8_dt(lo, p.dt);
-          if (n0 + c + 8 < p.CoutStore) reinterpret_cast<uint4*>(o)[1] = pack8_dt(hi, p.dt);
-        }
-      } else if (p.out_mode == 2) {
-        if (n0 + c < p.CoutStore) {
-          float4* o = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + (((long long)n * p.H + gy) * p.W + gx) * p.CoutStore + n0 + c);
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (n0 + c + 4 * j < p.CoutStore) o[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        }
-      } else {
-        float* o = reinterpret_cast<float*>(p.out);
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (n0 + c + j < p.CoutStore) o[(((long long)n * p.CoutStore + n0 + c + j) * p.H + gy) * p.W + gx] = v[j];
-      }
+    for (int j = 0; j < NT / 8; ++j) {
+      const int c = n0 + 8 * j + frag_col(t);
+      float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+      if (p.out_scale) { v0 *= sc; v1 *= sc; }
+      if (p.bias) { v0 += p.bias[c]; v1 += p.bias[c + 1]; }
+      store_pair(p.out, p.out_mode, p.dt, p.CoutStore, p.H, p.W, n, gy, gx, c, v0, v1);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -432,70 +350,26 @@ int dispatch_nt(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap&
 //
 //   * pixel tile = 8 w x (16*MT) h  (MT accumulators of M = 128 rows, row m = h*8 + w);
 //   * A: one TMA box (KBLK channels x 10 w x (16*MT+2) h) per k-block -- the 3x3 halo.  The nine taps are NOT
-//     reloaded: tap (dy,dx) of sub-tile j is the same shared-memory tile viewed through a UMMA descriptor whose
+//     reloaded: tap (dy,dx) of sub-tile j is the same shared-memory tile viewed through a wgmma descriptor whose
 //     start address is shifted by ((16*j+dy)*10 + dx) rows and whose 8-row-group stride (SBO) is one halo row
 //     (10 pixels).  The 128B/64B/32B swizzle is a function of the absolute shared-memory address (TMA writes and
-//     tcgen05 reads agree), so a row-shifted start keeps the pattern consistent.
+//     wgmma reads agree), so a row-shifted start keeps the pattern consistent.
 //   * B: the CTA's whole weight slice [taps][k-blocks][NT x KBLK] is loaded once (it fits: NT is chosen on the
 //     host so that taps*Cin*NT*2 <= ~148 KB) and stays resident while the CTA walks its pixel tiles.
-//   * TMEM: two sets of MT*NT fp32 columns; the epilogue of tile i overlaps the MMAs of tile i+1.
+//   * accumulators: MT x NT fp32 per 128 rows, i.e. MT*NT/2 registers per consumer thread (the host keeps MT*NT <= 128).
 // L2->SM traffic per output pixel drops from 9*(Cin + NT)*2 B (v1) to ~1.4*Cin*2 B.
 // ================================================================================================
-template <int SW>
-__device__ __forceinline__ uint64_t make_kmajor_desc_sbo(uint32_t saddr, uint32_t sbo_bytes, int base_offset_mode) {
-  constexpr uint64_t layout = (SW == 128) ? 2 : (SW == 64) ? 4 : 6;
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3ffff) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  if (base_offset_mode) d |= (uint64_t)((saddr >> 7) & 7) << 49;
-  d |= layout << 61;
-  return d;
-}
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
 struct ConvV2Params {
   int N, H, W;
   int C0, C1;
   int CoutP, CoutStore;
   int tiles_x, tiles_y, ntiles;
   int out_mode;
-  int desc_mode;
   int dt;                 // 16-bit operand / storage type: 0 bf16, 2 fp16
   const float* bias;
   void* out;
-  float* stat_partials;   // optional [gridDim.x][2][CoutP]: per-CTA sum / sum of squares of the stored (bf16-rounded) outputs
+  float* stat_partials;   // optional [gridDim.x][2][CoutP]: per-CTA sum / sum of squares of the stored (16-bit-rounded) outputs
 };
-
-// Sum over the 32 lanes of a warp for 16 per-lane values with a transpose-reduction (16 shuffles instead of 80):
-// returns, on every lane, the total of value index ((lane >> 1) & 15).
-__device__ __forceinline__ float warp_transpose_sum16(const float (&x)[16], int lane) {
-  float y[8], z[4], w[2];
-  const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4, h2 = lane & 2;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float send = h16 ? x[i] : x[i + 8], keep = h16 ? x[i + 8] : x[i];
-    y[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float send = h8 ? y[i] : y[i + 4], keep = h8 ? y[i + 4] : y[i];
-    z[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-  }
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const float send = h4 ? z[i] : z[i + 2], keep = h4 ? z[i + 2] : z[i];
-    w[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-  }
-  const float send = h2 ? w[0] : w[1], keep = h2 ? w[1] : w[0];
-  float r = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-  r += __shfl_xor_sync(0xffffffffu, r, 1);
-  return r;
-}
 
 template <int KS, int KBLK, int NT, int MT>
 struct ConvV2Cfg {
@@ -506,23 +380,49 @@ struct ConvV2Cfg {
   static constexpr int HALO_BYTES = HW_ * HH_ * ROWB;
   static constexpr int A_STAGE = ((HALO_BYTES + 1023) / 1024) * 1024;
   static constexpr int W_SUB = NT * ROWB;                  // one (tap, k-block) weight tile
-  static constexpr uint32_t TMEM_COLS = (2 * MT * NT <= 32) ? 32 : (2 * MT * NT <= 64) ? 64 : (2 * MT * NT <= 128) ? 128
-                                        : (2 * MT * NT <= 256) ? 256 : 512;
 };
 
-// conv_tc2 runs EIGHT epilogue warps (two per TMEM lane quarter, each taking half of the accumulator columns): the
-// epilogue (tcgen05.ld, bias, bf16 pack, stores, BatchNorm partial sums) was the pacing stage with four.
-template <int NT, int MT>
-struct Conv2Epi { static constexpr int WARPS = (NT >= 64 && MT == 1) ? 8 : 4; static constexpr int THREADS = 64 + 32 * WARPS; };
+// Per-thread running BatchNorm sums (NT/4 channels per thread: column 8*j + frag_col + b) -> this CTA's row of
+// stat_partials: the lanes holding the same channels are summed with shuffles, then the eight consumer warps in a
+// fixed order.  Consumer threads only (named barrier 1).
+template <int NT>
+__device__ __forceinline__ void write_stat_partials(float (&rs)[NT / 4], float (&rq)[NT / 4], float* stat_partials, int CoutP, int n0) {
+  __shared__ float s_stat[CONSUMER_WARPS][2][NT];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 0; k < NT / 4; ++k) {
+#pragma unroll
+    for (int o = 4; o < 32; o <<= 1) {
+      rs[k] += __shfl_xor_sync(0xffffffffu, rs[k], o);
+      rq[k] += __shfl_xor_sync(0xffffffffu, rq[k], o);
+    }
+  }
+  if (lane < 4) {
+#pragma unroll
+    for (int k = 0; k < NT / 4; ++k) {
+      const int ch = 8 * (k >> 1) + 2 * lane + (k & 1);
+      s_stat[warp][0][ch] = rs[k];
+      s_stat[warp][1][ch] = rq[k];
+    }
+  }
+  asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+  for (int c = threadIdx.x; c < 2 * NT; c += CONSUMERS) {
+    const int which = c / NT, ch = c % NT;
+    float a = 0.f;
+#pragma unroll
+    for (int w = 0; w < CONSUMER_WARPS; ++w) a += s_stat[w][which][ch];
+    stat_partials[((size_t)blockIdx.x * 2 + which) * CoutP + n0 + ch] = a;
+  }
+}
 
 template <int KS, int KBLK, int NT, int MT, int STAGES>
-__global__ void __launch_bounds__(Conv2Epi<NT, MT>::THREADS) conv_tc2_kernel(const __grid_constant__ CUtensorMap map_a0,
-                                                               const __grid_constant__ CUtensorMap map_a1,
-                                                               const __grid_constant__ CUtensorMap map_b, const ConvV2Params p,
-                                                               const int w_bytes) {
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc2_kernel(const __grid_constant__ CUtensorMap map_a0,
+                                                                  const __grid_constant__ CUtensorMap map_a1,
+                                                                  const __grid_constant__ CUtensorMap map_b, const ConvV2Params p,
+                                                                  const int w_bytes) {
   using Cfg = ConvV2Cfg<KS, KBLK, NT, MT>;
   constexpr int SW = KBLK * 2, T = KS * KS;
-  static_assert(2 * MT * NT <= 512, "TMEM budget");
+  static_assert(MT * NT <= 128, "accumulator registers");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* w_smem = smem;
@@ -530,10 +430,7 @@ __global__ void __launch_bounds__(Conv2Epi<NT, MT>::THREADS) conv_tc2_kernel(con
   uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + STAGES * Cfg::A_STAGE);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + STAGES;
-  uint64_t* acc_full = bars + 2 * STAGES;
-  uint64_t* acc_empty = bars + 2 * STAGES + 2;
-  uint64_t* w_bar = bars + 2 * STAGES + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 5);
+  uint64_t* w_bar = bars + 2 * STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n0 = blockIdx.y * NT;
@@ -541,20 +438,17 @@ __global__ void __launch_bounds__(Conv2Epi<NT, MT>::THREADS) conv_tc2_kernel(con
   const int my_tiles = (p.ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], Conv2Epi<NT, MT>::WARPS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], CONSUMER_WARPS); }
     mbar_init(w_bar, 1);
     fence_barrier_init();
     prefetch_tmap(&map_a0);
     prefetch_tmap(&map_b);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= PRODUCER_WARP) {
+    producer_regs();
+    if (warp != PRODUCER_WARP) return;
     if (lane == 0) {
       mbar_expect_tx(w_bar, (uint32_t)(T * nkb * Cfg::W_SUB));
       for (int t = 0; t < T; ++t)
@@ -574,161 +468,93 @@ __global__ void __launch_bounds__(Conv2Epi<NT, MT>::THREADS) conv_tc2_kernel(con
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = idesc_for(make_idesc_bf16(NT), p.dt);
-    constexpr uint32_t a_hi = desc_hi<SW>(Cfg::HW_ * Cfg::ROWB), b_hi = desc_hi<SW>(8 * SW);
-    const uint32_t elected = elect_one();
-    const uint32_t tmem_u = uniform(tmem_base);
-    const uint32_t a_lo0 = (uniform(smem_u32(a_smem)) >> 4) | 0x10000u;      // LBO field = 1 (ignored for swizzled K-major)
-    const uint32_t w_lo0 = (uniform(smem_u32(w_smem)) >> 4) | 0x10000u;
-    const uint32_t w_tap = (uint32_t)(nkb * Cfg::W_SUB) >> 4;               // descriptor units between two taps of the weights
-    mbar_wait(w_bar, 0);
-    int it = 0;
-    for (int i = 0; i < my_tiles; ++i) {
-      const int acc = i & 1;
-      mbar_wait(&acc_empty[acc], ((i >> 1) & 1) ^ 1);
-      tc_fence_after();
-      for (int kb = 0; kb < nkb; ++kb, ++it) {
-        const int s = it % STAGES;
-        mbar_wait(&a_full[s], (it / STAGES) & 1);
-        tc_fence_after();
-        if (elected) {
-          const uint32_t a_lo = a_lo0 + (uint32_t)(s * (Cfg::A_STAGE >> 4));
-          const uint32_t w_lo = w_lo0 + (uint32_t)(kb * (Cfg::W_SUB >> 4));
-          const uint32_t d0 = tmem_u + (uint32_t)(acc * MT * NT);
+    return;
+  }
+  consumer_regs();
+  const int h = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const uint32_t a_u = smem_u32(a_smem), w_u = smem_u32(w_smem);
+  float rs[NT / 4], rq[NT / 4];          // running per-channel sum / sum of squares of this thread's pixels
 #pragma unroll
-          for (int j = 0; j < MT; ++j) {
+  for (int k = 0; k < NT / 4; ++k) rs[k] = rq[k] = 0.f;
+  mbar_wait(w_bar, 0);
+  int it = 0;
+  for (int i = 0; i < my_tiles; ++i) {
+    const int tile = blockIdx.x + i * gridDim.x;
+    const int n = tile / (p.tiles_x * p.tiles_y);
+    const int tr = tile - n * p.tiles_x * p.tiles_y;
+    const int y0 = (tr / p.tiles_x) * Cfg::TH, x0 = (tr % p.tiles_x) * Cfg::TW;
+    float acc[MT][NT / 2];
 #pragma unroll
-            for (int t = 0; t < T; ++t) {
-              const int dy = t / KS, dx = t % KS;
+    for (int j = 0; j < MT; ++j)
 #pragma unroll
-              for (int k = 0; k < KBLK / 16; ++k)
-                umma_f16_w(d0 + (uint32_t)(j * NT), a_lo + (uint32_t)(((((16 * j + dy) * Cfg::HW_ + dx) * Cfg::ROWB) >> 4) + 2 * k), a_hi,
-                           w_lo + (uint32_t)t * w_tap + (uint32_t)(2 * k), b_hi, idesc, (kb > 0 || t > 0 || k > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(&a_empty[s]);
-          if (kb == nkb - 1) umma_commit(&acc_full[acc]);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    constexpr int NCH = NT / 16;                           // 16-column chunks of the accumulator
-    constexpr int EW = Conv2Epi<NT, MT>::WARPS;
-    const int half = (warp - 2) >> 2;                      // which half of the chunks this warp owns (EW == 8)
-    const int ch_lo = (EW == 8) ? half * (NCH / 2) : 0;
-    const int ch_hi = (EW == 8) ? (half + 1) * (NCH / 2) : NCH;
-    float rs[NT / 16], rq[NT / 16];       // running per-channel sum / sum of squares (channel = chunk*16 + ((lane>>1)&15))
+      for (int e = 0; e < NT / 2; ++e) acc[j][e] = 0.f;
+    for (int kb = 0; kb < nkb; ++kb, ++it) {
+      const int s = it % STAGES;
+      mbar_wait(&a_full[s], (it / STAGES) & 1);
+      // rows 64h.. of a sub-tile start 8h halo rows further down
+      const uint32_t a_base = a_u + (uint32_t)(s * Cfg::A_STAGE + 8 * h * Cfg::HW_ * Cfg::ROWB);
+      const uint32_t w_base = w_u + (uint32_t)(kb * Cfg::W_SUB);
+      wgmma_fence();
 #pragma unroll
-    for (int c = 0; c < NT / 16; ++c) rs[c] = rq[c] = 0.f;
-    for (int i = 0; i < my_tiles; ++i) {
-      const int tile = blockIdx.x + i * gridDim.x;
-      const int n = tile / (p.tiles_x * p.tiles_y);
-      const int tr = tile - n * p.tiles_x * p.tiles_y;
-      const int y0 = (tr / p.tiles_x) * Cfg::TH, x0 = (tr % p.tiles_x) * Cfg::TW;
-      const int acc = i & 1;
-      mbar_wait(&acc_full[acc], (i >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
       for (int j = 0; j < MT; ++j) {
+#pragma unroll
+        for (int tap = 0; tap < T; ++tap) {
+          const int dy = tap / KS, dx = tap % KS;
+#pragma unroll
+          for (int k = 0; k < KBLK / 16; ++k)
+            Wgmma<NT>::template mma<0, 0>(acc[j],
+                                          gmma_desc<SW>(a_base + (uint32_t)(((16 * j + dy) * Cfg::HW_ + dx) * Cfg::ROWB + 32 * k), 16, Cfg::HW_ * Cfg::ROWB),
+                                          gmma_desc<SW>(w_base + (uint32_t)(tap * nkb * Cfg::W_SUB + 32 * k), 16, 8 * SW),
+                                          (kb > 0 || tap > 0 || k > 0) ? 1u : 0u, p.dt);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      release_stage(&a_empty[s]);
+    }
+#pragma unroll
+    for (int j = 0; j < MT; ++j) {
+      wgmma_fence_regs(acc[j]);
+#pragma unroll
+      for (int ii = 0; ii < 2; ++ii) {
+        const int m = 64 * h + frag_row(t) + 8 * ii;
         const int gy = y0 + 16 * j + m / 8, gx = x0 + (m & 7);
 #pragma unroll
-        for (int c = 0; c < NT; c += 16) {
-          if (c / 16 < ch_lo || c / 16 >= ch_hi) continue;   // warp-uniform: the other epilogue warp of this quarter owns it
-          float v[16];
-          tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((acc * MT + j) * NT + c), v);
-          if (p.bias) {
-#pragma unroll
-            for (int jj = 0; jj < 16; ++jj) v[jj] += p.bias[n0 + c + jj];
+        for (int jj = 0; jj < NT / 8; ++jj) {
+          const int c = 8 * jj + frag_col(t);
+          float v0 = acc[j][4 * jj + 2 * ii], v1 = acc[j][4 * jj + 2 * ii + 1];
+          if (p.bias) { v0 += p.bias[n0 + c]; v1 += p.bias[n0 + c + 1]; }
+          if (p.out_mode == 0 && p.stat_partials) {   // BatchNorm statistics of the values exactly as stored
+            float2 r;
+            if (p.dt == 2) r = __half22float2(__floats2half2_rn(v0, v1));
+            else r = __bfloat1622float2(__floats2bfloat162_rn(v0, v1));
+            rs[2 * jj] += r.x;     rq[2 * jj] += r.x * r.x;
+            rs[2 * jj + 1] += r.y; rq[2 * jj + 1] += r.y * r.y;
           }
-          if (p.out_mode == 0) {
-            float lo[8], hi[8];
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) { lo[jj] = v[jj]; hi[jj] = v[8 + jj]; }
-            const uint4 plo = pack8_dt(lo, p.dt), phi = pack8_dt(hi, p.dt);
-            if (n0 + c < p.CoutStore) {
-              __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + (((long long)n * p.H + gy) * p.W + gx) * p.CoutStore + n0 + c;
-              reinterpret_cast<uint4*>(o)[0] = plo;
-              if (n0 + c + 8 < p.CoutStore) reinterpret_cast<uint4*>(o)[1] = phi;
-            }
-            if (p.stat_partials) {   // BatchNorm statistics of the values exactly as stored (rounded to the 16-bit type)
-              float r[16], r2[16];
-              unpack8_dt(plo, lo, p.dt);
-              unpack8_dt(phi, hi, p.dt);
-#pragma unroll
-              for (int jj = 0; jj < 8; ++jj) { r[jj] = lo[jj]; r[8 + jj] = hi[jj]; }
-#pragma unroll
-              for (int jj = 0; jj < 16; ++jj) r2[jj] = r[jj] * r[jj];
-              rs[c / 16] += warp_transpose_sum16(r, lane);
-              rq[c / 16] += warp_transpose_sum16(r2, lane);
-            }
-          } else {
-            float* o = reinterpret_cast<float*>(p.out);
-#pragma unroll
-            for (int jj = 0; jj < 16; ++jj)
-              if (n0 + c + jj < p.CoutStore) o[(((long long)n * p.CoutStore + n0 + c + jj) * p.H + gy) * p.W + gx] = v[jj];
-          }
+          store_pair(p.out, p.out_mode == 0 ? 0 : 1, p.dt, p.CoutStore, p.H, p.W, n, gy, gx, n0 + c, v0, v1);
         }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[acc]);
-    }
-    if (p.stat_partials) {
-      // combine the four epilogue warps (fixed order) and write this CTA's partial row
-      __shared__ float s_stat[4][2][NT];
-      if ((lane & 1) == 0) {
-#pragma unroll
-        for (int c = 0; c < NT / 16; ++c) {
-          if (c < ch_lo || c >= ch_hi) continue;
-          s_stat[q][0][c * 16 + ((lane >> 1) & 15)] = rs[c];
-          s_stat[q][1][c * 16 + ((lane >> 1) & 15)] = rq[c];
-        }
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
-      const int t = threadIdx.x - 64;      // index over the epilogue warps
-      for (int c = t; c < 2 * NT; c += 32 * EW) {
-        const int which = c / NT, ch = c % NT;
-        const float a = ((s_stat[0][which][ch] + s_stat[1][which][ch]) + s_stat[2][which][ch]) + s_stat[3][which][ch];
-        p.stat_partials[((size_t)blockIdx.x * 2 + which) * p.CoutP + n0 + ch] = a;
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  if (p.out_mode == 0 && p.stat_partials) write_stat_partials<NT>(rs, rq, p.stat_partials, p.CoutP, n0);
 }
 
 // ================================================================================================
-// tcgen05 weight gradient:  dW[co][ci][t] += sum_{pixels} dY[p][co] * X[p + tap_t][ci]
+// wgmma weight gradient:  dW[co][ci][t] += sum_{pixels} dY[p][co] * X[p + tap_t][ci]
 //
-//   D_t[M = 128 couts, N = CWB cins] (fp32, TMEM) += A^T[K = 128 pixels x M] * B_t[K = 128 pixels x N]
+//   D_t[M = 128 couts, N = CWB cins] (fp32, registers) += A^T[K = 128 pixels x M] * B_t[K = 128 pixels x N]
 //
 // Both operands are "MN-major" for the tensor core: K (pixels) indexes shared-memory rows, the channel (M or N)
 // is contiguous inside a row -- exactly what a channels-last TMA box (channels x 16 w x 8 h) produces.  A (dY) is
 // loaded once per 128-pixel chunk, B (the tap-shifted X box, TMA zero fill = padding) once per tap of the CTA's
 // tap group; each CTA owns (Cout tile of 128) x (Cin block of CWB) x (TG taps), loops over its share of the
-// N*H*W/128 pixel chunks (split-K), keeps TG accumulators in TMEM and finally adds them into the fp32
+// N*H*W/128 pixel chunks (split-K), keeps TG accumulators in registers and finally adds them into the fp32
 // torch-layout gradient with red.global.add.f32.
 //   CWA/CWB = channels per A/B box (16/32/64 -> swizzle 32/64/128 B), NA = A boxes per stage (1 or 2).
-// When Cout < 128 the MMA still runs M = 128 (same tensor-pipe cost as M = 64): the missing row groups alias
-// whatever shared memory follows the A box; those accumulator rows are never read.
+// Consumer warpgroup h owns couts 64h..64h+63 of the tile and skips its MMAs when they are all padding.  When Cout < 64
+// the M = 64 MMA still reads the missing channel groups from whatever shared memory follows the A box; those
+// accumulator rows are never stored.
 // ================================================================================================
-template <int SW>
-__device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t saddr, uint32_t lbo_bytes) {
-  constexpr uint64_t layout = (SW == 128) ? 2 : (SW == 64) ? 4 : 6;
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3ffff) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;   // stride between SW-byte wide channel groups
-  d |= (uint64_t)((8 * SW) >> 4) << 32;                // stride between 8-pixel row groups
-  d |= (uint64_t)1 << 46;
-  d |= layout << 61;
-  return d;
-}
-
 struct WgradTcParams {
   int N, H, W;
   int C0, C1;          // source channels
@@ -750,7 +576,7 @@ struct WgradSmem {
   static constexpr int A_BOX = TILE_M * CWA * 2;
   static constexpr int B_BOX = TILE_M * CWB * 2;
   static constexpr int STAGE_BYTES = ((NA * A_BOX + TG * B_BOX + 1023) / 1024) * 1024;
-  static constexpr int SLACK = (128 / CWA) * A_BOX;   // aliased row groups of the last stage stay inside the allocation
+  static constexpr int SLACK = (64 / CWA) * A_BOX;    // aliased channel groups of the last stage stay inside the allocation
   static constexpr int TOTAL = STAGES * STAGE_BYTES + SLACK + 1024 + 256;
 };
 
@@ -760,13 +586,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const __grid_c
                                                                   const __grid_constant__ CUtensorMap map_x1, const WgradTcParams p) {
   using S = WgradSmem<CWA, NA, CWB, TG, STAGES>;
   constexpr int SWA = CWA * 2, SWB = CWB * 2;
-  constexpr uint32_t TMEM_COLS = (TG * CWB <= 32) ? 32 : (TG * CWB <= 64) ? 64 : (TG * CWB <= 128) ? 128 : 256;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES + S::SLACK);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // blockIdx.y -> (m tile, n tile, tap group)
@@ -783,19 +606,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const __grid_c
   const int my_chunks = (p.nchunks - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_WARPS); }
     fence_barrier_init();
     prefetch_tmap(&map_dy);
     prefetch_tmap(src1 ? &map_x1 : &map_x0);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= PRODUCER_WARP) {
+    producer_regs();
+    if (warp != PRODUCER_WARP) return;
     if (lane == 0) {
       const CUtensorMap* mx = src1 ? &map_x1 : &map_x0;
       for (int it = 0; it < my_chunks; ++it) {
@@ -819,73 +639,62 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = idesc_for(make_idesc_bf16(CWB, /*a_mn_major=*/1, /*b_mn_major=*/1, 128), p.dt);
-    for (int it = 0; it < my_chunks; ++it) {
-      const int s = it % STAGES;
-      const uint32_t ph = (it / STAGES) & 1;
-      mbar_wait(&full_bar[s], ph);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES);
-        const uint32_t b_addr = a_addr + NA * S::A_BOX;
-        const uint64_t adesc = make_mnmajor_desc<SWA>(a_addr, S::A_BOX);
+    return;
+  }
+  consumer_regs();
+  const int h = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const bool active = m0 + 64 * h < p.CoutP;
+  float acc[TG][CWB / 2];
 #pragma unroll
-        for (int tl = 0; tl < TG; ++tl) {
-          const uint64_t bdesc = make_mnmajor_desc<SWB>(b_addr + tl * S::B_BOX, S::B_BOX);
+  for (int tl = 0; tl < TG; ++tl)
 #pragma unroll
-          for (int k = 0; k < TILE_M / 16; ++k) {
-            // 16 pixels (rows) per MMA: advance both operands by 16 rows
-            umma_f16(tmem_base + tl * CWB, adesc + (uint64_t)((k * 16 * SWA) >> 4), bdesc + (uint64_t)((k * 16 * SWB) >> 4), idesc,
-                     (it > 0 || k > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (it == my_chunks - 1) umma_commit(accum_bar);
+    for (int e = 0; e < CWB / 2; ++e) acc[tl][e] = 0.f;
+  for (int it = 0; it < my_chunks; ++it) {
+    const int s = it % STAGES;
+    mbar_wait(&full_bar[s], (it / STAGES) & 1);
+    if (active) {
+      const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES) + (uint32_t)((64 * h / CWA) * S::A_BOX);
+      const uint32_t b_addr = smem_u32(smem + s * S::STAGE_BYTES + NA * S::A_BOX);
+      wgmma_fence();
+#pragma unroll
+      for (int tl = 0; tl < TG; ++tl) {
+#pragma unroll
+        for (int k = 0; k < TILE_M / 16; ++k)   // 16 pixels (rows) per MMA: advance both operands by 16 rows
+          Wgmma<CWB>::template mma<1, 1>(acc[tl], gmma_desc<SWA>(a_addr + (uint32_t)(k * 16 * SWA), S::A_BOX, 8 * SWA),
+                                         gmma_desc<SWB>(b_addr + (uint32_t)(tl * S::B_BOX + k * 16 * SWB), S::B_BOX, 8 * SWB),
+                                         (it > 0 || k > 0) ? 1u : 0u, p.dt);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>();
     }
-  } else if (my_chunks > 0) {
-    const int q = warp & 3;
-    const int row = m0 + q * 32 + lane;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const int CinTot = p.C0 + p.C1;
-    const float osc = (p.scale_a ? *p.scale_a : 1.f) * (p.scale_b ? *p.scale_b : 1.f);
-    if (p.partials != nullptr) {          // deterministic split-K (see wgrad1_finalize_kernel)
-      float* slot = p.partials + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * (size_t)(TG * CWB * 128) + (q * 32 + lane);
-#pragma unroll 1
-      for (int c = 0; c < TG * CWB; c += 16) {
-        float v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
+    release_stage(&empty_bar[s]);
+  }
+  if (my_chunks == 0 || !active) return;
+  const int CinTot = p.C0 + p.C1;
+  const float osc = (p.scale_a ? *p.scale_a : 1.f) * (p.scale_b ? *p.scale_b : 1.f);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) slot[(size_t)(c + j) * 128] = v[j] * osc;
-      }
-    } else
-#pragma unroll 1
-    for (int tl = 0; tl < TG; ++tl) {
-      const int t = tg * TG + tl;
-#pragma unroll 1
-      for (int c = 0; c < CWB; c += 16) {
-        float v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(tl * CWB + c), v);
-        if (row < p.CoutReal && q * 32 + lane < 128) {
-          float* dst = p.dw + ((size_t)row * CinTot + ci_global + c) * p.taps + t;
+  for (int tl = 0; tl < TG; ++tl) {
+    wgmma_fence_regs(acc[tl]);
 #pragma unroll
-          for (int j = 0; j < 16; ++j) atomicAdd(dst + (size_t)j * p.taps, v[j] * osc);
-        }
+    for (int ii = 0; ii < 2; ++ii) {
+      const int r = 64 * h + frag_row(t) + 8 * ii, row = m0 + r;   // output channel
+#pragma unroll
+      for (int e = 0; e < CWB / 4; ++e) {
+        const int c = 8 * (e >> 1) + frag_col(t) + (e & 1);          // input channel inside the block
+        const float v = acc[tl][4 * (e >> 1) + 2 * ii + (e & 1)] * osc;
+        if (p.partials != nullptr)          // deterministic split-K (see wgrad1_finalize_kernel)
+          p.partials[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * (size_t)(TG * CWB * 128) + (size_t)(tl * CWB + c) * 128 + r] = v;
+        else if (row < p.CoutReal)
+          atomicAdd(p.dw + ((size_t)row * CinTot + ci_global + c) * p.taps + tg * TG + tl, v);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // ================================================================================================
 // wgrad v2 (3x3 only): one halo load of X per 8x16 pixel chunk; the nine tap operands are row-shifted MN-major
 // descriptor views of that halo (same absolute-address swizzle argument as conv_tc2).  CTA = (Cout tile of 128) x
-// (Cin block of CWB <= 32) x all nine taps -> nine accumulators of CWB columns in TMEM (<= 288 columns).
+// (Cin block of CWB <= 32) x all nine taps -> nine accumulators of CWB columns (9*CWB/2 registers per consumer thread).
 // L2->SM traffic per chunk: dY tile + 1.4x X block instead of dY + 9 X boxes.
 // ================================================================================================
 template <int CWA, int NA, int CWB, int STAGES>
@@ -894,21 +703,9 @@ struct Wgrad2Smem {
   static constexpr int ROWB = CWB * 2;
   static constexpr int B_HALO = ((10 * 18 * ROWB + 1023) / 1024) * 1024;
   static constexpr int STAGE_BYTES = ((NA * A_BOX + B_HALO + 1023) / 1024) * 1024;
-  static constexpr int SLACK = (128 / CWA) * A_BOX;
+  static constexpr int SLACK = (64 / CWA) * A_BOX;
   static constexpr int TOTAL = STAGES * STAGE_BYTES + SLACK + 1024 + 256;
 };
-
-template <int SW>
-__device__ __forceinline__ uint64_t make_mnmajor_desc_sbo(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  constexpr uint64_t layout = (SW == 128) ? 2 : (SW == 64) ? 4 : 6;
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3ffff) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= layout << 61;
-  return d;
-}
 
 template <int CWA, int NA, int CWB, int STAGES>
 __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc2_kernel(const __grid_constant__ CUtensorMap map_dy,
@@ -916,13 +713,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc2_kernel(const __grid_
                                                                    const __grid_constant__ CUtensorMap map_x1, const WgradTcParams p) {
   using S = Wgrad2Smem<CWA, NA, CWB, STAGES>;
   constexpr int SWA = CWA * 2, SWB = CWB * 2;
-  constexpr uint32_t TMEM_COLS = (9 * CWB <= 256) ? 256 : 512;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES + S::SLACK);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = p.n_tiles0 + p.n_tiles1;
@@ -935,19 +729,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc2_kernel(const __grid_
   const int my_chunks = (p.nchunks - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_WARPS); }
     fence_barrier_init();
     prefetch_tmap(&map_dy);
     prefetch_tmap(src1 ? &map_x1 : &map_x0);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= PRODUCER_WARP) {
+    producer_regs();
+    if (warp != PRODUCER_WARP) return;
     if (lane == 0) {
       const CUtensorMap* mx = src1 ? &map_x1 : &map_x0;
       for (int it = 0; it < my_chunks; ++it) {
@@ -965,55 +756,54 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc2_kernel(const __grid_
         tma_load_4d(mx, &full_bar[s], b_dst, cb0, x0 - 1, y0 - 1, n);
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = idesc_for(make_idesc_bf16(CWB, 1, 1, 128), p.dt);
-    for (int it = 0; it < my_chunks; ++it) {
-      const int s = it % STAGES;
-      mbar_wait(&full_bar[s], (it / STAGES) & 1);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES);
-        const uint32_t b_addr = a_addr + NA * S::A_BOX;
-        const uint64_t adesc = make_mnmajor_desc_sbo<SWA>(a_addr, S::A_BOX, 8 * SWA);
+    return;
+  }
+  consumer_regs();
+  const int h = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const bool active = m0 + 64 * h < p.CoutP;
+  float acc[9][CWB / 2];
 #pragma unroll
-        for (int t = 0; t < 9; ++t) {
-          const int dy = t / 3, dx = t % 3;
-          const uint64_t bdesc = make_mnmajor_desc_sbo<SWB>(b_addr + (uint32_t)((dy * 10 + dx) * S::ROWB), S::B_HALO, 10 * S::ROWB);
+  for (int tap = 0; tap < 9; ++tap)
 #pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            // k-step = 16 pixels = image rows 2k, 2k+1 of the chunk: A advances 16 rows, B advances 2 halo rows
-            umma_f16(tmem_base + t * CWB, adesc + (uint64_t)((k * 16 * SWA) >> 4), bdesc + (uint64_t)((k * 2 * 10 * S::ROWB) >> 4), idesc,
-                     (it > 0 || k > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (it == my_chunks - 1) umma_commit(accum_bar);
+    for (int e = 0; e < CWB / 2; ++e) acc[tap][e] = 0.f;
+  for (int it = 0; it < my_chunks; ++it) {
+    const int s = it % STAGES;
+    mbar_wait(&full_bar[s], (it / STAGES) & 1);
+    if (active) {
+      const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES) + (uint32_t)((64 * h / CWA) * S::A_BOX);
+      const uint32_t b_addr = smem_u32(smem + s * S::STAGE_BYTES + NA * S::A_BOX);
+      wgmma_fence();
+#pragma unroll
+      for (int tap = 0; tap < 9; ++tap) {
+        const int dy = tap / 3, dx = tap % 3;
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          // k-step = 16 pixels = image rows 2k, 2k+1 of the chunk: A advances 16 rows, B advances 2 halo rows
+          Wgmma<CWB>::template mma<1, 1>(acc[tap], gmma_desc<SWA>(a_addr + (uint32_t)(k * 16 * SWA), S::A_BOX, 8 * SWA),
+                                         gmma_desc<SWB>(b_addr + (uint32_t)((dy * 10 + dx) * S::ROWB + k * 2 * 10 * S::ROWB), S::B_HALO, 10 * S::ROWB),
+                                         (it > 0 || k > 0) ? 1u : 0u, p.dt);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>();
     }
-  } else if (my_chunks > 0) {
-    const int q = warp & 3;
-    const int row = m0 + q * 32 + lane;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const int CinTot = p.C0 + p.C1;
-#pragma unroll 1
-    for (int t = 0; t < 9; ++t) {
-#pragma unroll 1
-      for (int c = 0; c < CWB; c += 16) {
-        float v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(t * CWB + c), v);
-        if (row < p.CoutReal) {
-          float* dst = p.dw + ((size_t)row * CinTot + ci_global + c) * 9 + t;
+    release_stage(&empty_bar[s]);
+  }
+  if (my_chunks == 0 || !active) return;
+  const int CinTot = p.C0 + p.C1;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) atomicAdd(dst + (size_t)j * 9, v[j]);
-        }
+  for (int tap = 0; tap < 9; ++tap) {
+    wgmma_fence_regs(acc[tap]);
+#pragma unroll
+    for (int ii = 0; ii < 2; ++ii) {
+      const int row = m0 + 64 * h + frag_row(t) + 8 * ii;
+      if (row >= p.CoutReal) continue;
+#pragma unroll
+      for (int e = 0; e < CWB / 4; ++e) {
+        const int c = 8 * (e >> 1) + frag_col(t) + (e & 1);
+        atomicAdd(p.dw + ((size_t)row * CinTot + ci_global + c) * 9 + tap, acc[tap][4 * (e >> 1) + 2 * ii + (e & 1)]);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 template <int CWA, int NA, int CWB>
@@ -1029,7 +819,7 @@ int launch_wgrad2(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensor
     attr = true;
   }
   const int gy = m_tiles * (p.n_tiles0 + p.n_tiles1);
-  int splits = (148 + gy - 1) / gy;
+  int splits = (wsl_num_sms() + gy - 1) / gy;
   if (splits > p.nchunks) splits = p.nchunks;
   if (splits < 1) splits = 1;
   dim3 grid(splits, gy);
@@ -1038,28 +828,24 @@ int launch_wgrad2(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensor
 }
 
 // ================================================================================================
-// wgrad v3 (3x3): taps in the M dimension.
+// wgrad v3 (3x3): taps in the M dimension, filter rows in the N dimension.
 //
-//   A := X halo (MN-major).  An M = 128 operand is 128/CWB channel groups spaced LBO apart; with LBO = ONE PIXEL
-//        (CWB*2 bytes) group g is the same halo viewed g pixels further right, i.e. filter column dx = g.  One MMA
-//        therefore accumulates dx = 0,1,2 of a filter row at once (groups >= 3 are don't-care rows of D).
-//   B := dY tile (MN-major), N = the Cout tile (<= 128) -> wide N keeps the tensor pipe ahead of the A smem reads.
-//   D_dy[(dx, ci)][co], dy = 0..2: three accumulators of N columns in TMEM.
-// MMAs per 128-pixel chunk and 32-channel Cin block: 3 dy x 8 k-steps = 24 (v2 issued 72 narrow ones).
+//   A := X rows (MN-major).  An M = 64 operand is 64/CWB channel groups spaced LBO apart; with LBO = ONE PIXEL
+//        (CWB*2 bytes) group g is the same tile viewed g pixels further right, i.e. filter column dx = g.  One MMA
+//        therefore accumulates dx = 0,1,2 of the filter at once (groups >= 3 are don't-care rows of D; warpgroup 1,
+//        holding groups 64/CWB.., only runs when CWB = 32).
+//   B := dY tile (MN-major) loaded with one halo row above and below (18 x 8 pixels); N-group g of the B operand is
+//        the dY tile viewed g - 1 rows further down (LBO = one tile row), while A is the un-shifted X row block
+//        (16 x 10 pixels).  X[p + (1 - g) rows + dx] * dY[p] lands in column group g, i.e. dy = 2 - g; the products
+//        that fall outside the chunk's rows are exactly those against the zero padding (TMA zero fill).
+//   D[(dx, ci)][(dy, co)]: one accumulator of N = 3*NTILE columns (NTILE = Cout tile <= 64).
 // ================================================================================================
-// DYN (NBOX == 1 only): the filter ROWS go into the MMA's N dimension as well.  dY is loaded with one halo row above and below
-// (18 x 8 pixels); N-group g of the B operand is the dY tile viewed g - 1 rows further down (LBO = one tile row), while A is
-// the un-shifted X row block (16 x 10 pixels, LBO = one pixel -> filter column in M).  X[p + (1 - g) rows + dx] * dY[p] lands
-// in column group g, i.e. dy = 2 - g; the products that fall outside the chunk's rows are exactly those against the zero
-// padding (TMA zero fill).  One N = 3*NTILE MMA replaces three N = NTILE ones: 8 instead of 24 per chunk; with the measured
-// issue cost 10 + 32 (A read) + N/2 cycles that is 528 instead of 1224 cycles per chunk for the 16-channel layers.
-template <int CWB, int CWN, int NBOX, int STAGES, bool DYN>
+template <int CWB, int NTILE, int STAGES>
 struct Wgrad3Smem {
   static constexpr int ROWB = CWB * 2;
-  static constexpr int N_ROWS = DYN ? 18 : 16, X_ROWS = DYN ? 16 : 18;
-  static constexpr int N_BOX = N_ROWS * 8 * CWN * 2;
-  static constexpr int A_OFF = ((NBOX * N_BOX + 1023) / 1024) * 1024;
-  static constexpr int A_BYTES = 10 * X_ROWS * ROWB;
+  static constexpr int N_BOX = 18 * 8 * NTILE * 2;
+  static constexpr int A_OFF = ((N_BOX + 1023) / 1024) * 1024;
+  static constexpr int A_BYTES = 10 * 16 * ROWB;
   static constexpr int STAGE_BYTES = ((A_OFF + A_BYTES + 1023) / 1024) * 1024;
   static constexpr int SLACK = 2048;
   static constexpr int TOTAL = STAGES * STAGE_BYTES + SLACK + 1024 + 256;
@@ -1076,21 +862,16 @@ struct Wgrad3Params {
   float* partials;            // optional [gridDim.y][gridDim.x][3*NTILE][128]: per-CTA partial tiles for the fixed-order finalize
 };
 
-template <int CWB, int CWN, int NBOX, int STAGES, bool DYN>
-__global__ void __launch_bounds__(NUM_THREADS, (DYN && CWN <= 32) ? 2 : 1) wgrad_tc3_kernel(const __grid_constant__ CUtensorMap map_dy,
+template <int CWB, int NTILE, int STAGES>
+__global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc3_kernel(const __grid_constant__ CUtensorMap map_dy,
                                                                    const __grid_constant__ CUtensorMap map_x0,
                                                                    const __grid_constant__ CUtensorMap map_x1, const Wgrad3Params p) {
-  using S = Wgrad3Smem<CWB, CWN, NBOX, STAGES, DYN>;
-  static_assert(!DYN || NBOX == 1, "row merging needs a single dY box");
-  constexpr int NTILE = CWN * NBOX;
-  constexpr int SWX = CWB * 2, SWN = CWN * 2;
-  constexpr uint32_t TMEM_COLS = (3 * NTILE <= 64) ? 64 : (3 * NTILE <= 128) ? 128 : (3 * NTILE <= 256) ? 256 : 512;
+  using S = Wgrad3Smem<CWB, NTILE, STAGES>;
+  constexpr int SWX = CWB * 2, SWN = NTILE * 2, NG = 3 * NTILE;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES + S::SLACK);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k_tiles = p.k_tiles0 + p.k_tiles1;
@@ -1103,19 +884,16 @@ __global__ void __launch_bounds__(NUM_THREADS, (DYN && CWN <= 32) ? 2 : 1) wgrad
   const int my_chunks = (p.nchunks - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_WARPS); }
     fence_barrier_init();
     prefetch_tmap(&map_dy);
     prefetch_tmap(src1 ? &map_x1 : &map_x0);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= PRODUCER_WARP) {
+    producer_regs();
+    if (warp != PRODUCER_WARP) return;
     if (lane == 0) {
       const CUtensorMap* mx = src1 ? &map_x1 : &map_x0;
       for (int it = 0; it < my_chunks; ++it) {
@@ -1125,89 +903,58 @@ __global__ void __launch_bounds__(NUM_THREADS, (DYN && CWN <= 32) ? 2 : 1) wgrad
         const int y0 = (tr / p.tiles_x) * 16, x0 = (tr % p.tiles_x) * 8;
         const int s = it % STAGES;
         mbar_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
-        uint8_t* b_dst = smem + s * S::STAGE_BYTES;          // dY boxes
+        uint8_t* b_dst = smem + s * S::STAGE_BYTES;          // dY box
         uint8_t* a_dst = b_dst + S::A_OFF;                   // X block
-        mbar_expect_tx(&full_bar[s], NBOX * S::N_BOX + S::A_BYTES);
-#pragma unroll
-        for (int i = 0; i < NBOX; ++i)
-          tma_load_4d(&map_dy, &full_bar[s], b_dst + i * S::N_BOX, n0 + i * CWN, x0, DYN ? y0 - 1 : y0, n);
-        tma_load_4d(mx, &full_bar[s], a_dst, cb0, x0 - 1, DYN ? y0 : y0 - 1, n);
+        mbar_expect_tx(&full_bar[s], S::N_BOX + S::A_BYTES);
+        tma_load_4d(&map_dy, &full_bar[s], b_dst, n0, x0, y0 - 1, n);
+        tma_load_4d(mx, &full_bar[s], a_dst, cb0, x0 - 1, y0, n);
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = idesc_for(make_idesc_bf16(DYN ? 3 * NTILE : NTILE, 1, 1, 128), p.dt);
-    // A: channel-group stride (LBO) = one pixel, so group g == filter column dx = g; 8-pixel-row groups 10 halo pixels apart
-    constexpr uint32_t a_hi = desc_hi<SWX>(10 * S::ROWB), b_hi = desc_hi<SWN>(8 * SWN);
-    constexpr uint32_t a_lbo = ((uint32_t)(S::ROWB >> 4) & 0x3fffu) << 16;
-    constexpr uint32_t b_lbo = ((uint32_t)((DYN ? 8 * SWN : S::N_BOX) >> 4) & 0x3fffu) << 16;
-    const uint32_t elected = elect_one();
-    const uint32_t tmem_u = uniform(tmem_base);
-    const uint32_t s_lo0 = uniform(smem_u32(smem)) >> 4;
-    for (int it = 0; it < my_chunks; ++it) {
-      const int s = it % STAGES;
-      mbar_wait(&full_bar[s], (it / STAGES) & 1);
-      tc_fence_after();
-      if (elected) {
-        const uint32_t b_lo = (s_lo0 + (uint32_t)(s * (S::STAGE_BYTES >> 4))) | b_lbo;
-        const uint32_t a_lo = (s_lo0 + (uint32_t)(s * (S::STAGE_BYTES >> 4) + (S::A_OFF >> 4))) | a_lbo;
-        if constexpr (DYN) {
+    return;
+  }
+  consumer_regs();
+  const int h = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const bool active = 64 * h < 3 * CWB;       // warpgroup 1 holds filter columns only when the Cin block is 32 wide
+  float acc[NG / 2];
 #pragma unroll
-          for (int k = 0; k < 8; ++k)      // k-step = 16 pixels = chunk rows 2k, 2k+1
-            umma_f16_w(tmem_u, a_lo + (uint32_t)((k * 2 * 10 * S::ROWB) >> 4), a_hi, b_lo + (uint32_t)((k * 16 * SWN) >> 4), b_hi, idesc,
-                       (it > 0 || k > 0) ? 1u : 0u);
-        } else {
+  for (int e = 0; e < NG / 2; ++e) acc[e] = 0.f;
+  for (int it = 0; it < my_chunks; ++it) {
+    const int s = it % STAGES;
+    mbar_wait(&full_bar[s], (it / STAGES) & 1);
+    if (active) {
+      const uint32_t b_addr = smem_u32(smem + s * S::STAGE_BYTES);
+      const uint32_t a_addr = b_addr + (uint32_t)(S::A_OFF + (64 * h / CWB) * S::ROWB);
+      wgmma_fence();
 #pragma unroll
-          for (int dy = 0; dy < 3; ++dy) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-              umma_f16_w(tmem_u + (uint32_t)(dy * NTILE), a_lo + (uint32_t)(((dy * 10 * S::ROWB) >> 4) + ((k * 2 * 10 * S::ROWB) >> 4)), a_hi,
-                         b_lo + (uint32_t)((k * 16 * SWN) >> 4), b_hi, idesc, (it > 0 || k > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (it == my_chunks - 1) umma_commit(accum_bar);
-      }
-      __syncwarp();
+      for (int k = 0; k < 8; ++k)      // k-step = 16 pixels = chunk rows 2k, 2k+1
+        Wgmma<NG>::template mma<1, 1>(acc, gmma_desc<SWX>(a_addr + (uint32_t)(k * 2 * 10 * S::ROWB), S::ROWB, 10 * S::ROWB),
+                                      gmma_desc<SWN>(b_addr + (uint32_t)(k * 16 * SWN), 8 * SWN, 8 * SWN), (it > 0 || k > 0) ? 1u : 0u, p.dt);
+      wgmma_commit();
+      wgmma_wait<0>();
     }
-  } else if (my_chunks > 0) {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
+    release_stage(&empty_bar[s]);
+  }
+  if (my_chunks == 0 || !active) return;
+  wgmma_fence_regs(acc);
+  const int CinTot = p.C0 + p.C1;
+#pragma unroll
+  for (int ii = 0; ii < 2; ++ii) {
+    const int m = 64 * h + frag_row(t) + 8 * ii;
     const int g = m / CWB, ci = m % CWB;        // filter column dx, input channel inside the block
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const int CinTot = p.C0 + p.C1;
-    if (p.partials != nullptr) {
-      // deterministic split-K: this CTA's partial tile goes to its own slot (coalesced: lane = TMEM lane is the fastest index);
-      // wgrad3_finalize_kernel sums the slots of an output tile in split order and adds the result into dw
-      float* slot = p.partials + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * (size_t)(3 * NTILE * 128) + m;
-#pragma unroll 1
-      for (int c = 0; c < 3 * NTILE; c += 16) {
-        float v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) slot[(size_t)(c + j) * 128] = v[j];
-      }
-    } else
-#pragma unroll 1
-    for (int grp = 0; grp < 3; ++grp) {
-      const int dy = DYN ? 2 - grp : grp;       // column group -> filter row
-#pragma unroll 1
-      for (int c = 0; c < NTILE; c += 16) {
-        float v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(grp * NTILE + c), v);
-        if (g < 3) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int co = n0 + c + j;
-            if (co < p.CoutReal) atomicAdd(p.dw + ((size_t)co * CinTot + ci_global + ci) * 9 + dy * 3 + g, v[j]);
-          }
-        }
+    for (int e = 0; e < NG / 4; ++e) {
+      const int col = 8 * (e >> 1) + frag_col(t) + (e & 1);
+      const float v = acc[4 * (e >> 1) + 2 * ii + (e & 1)];
+      if (p.partials != nullptr) {
+        // deterministic split-K: this CTA's partial tile goes to its own slot; wgrad3_finalize_kernel sums the slots of an
+        // output tile in split order and adds the result into dw
+        p.partials[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * (size_t)(NG * 128) + (size_t)col * 128 + m] = v;
+      } else {
+        const int grp = col / NTILE, co = n0 + col % NTILE, dy = 2 - grp;   // column group -> filter row
+        if (g < 3 && co < p.CoutReal) atomicAdd(p.dw + ((size_t)co * CinTot + ci_global + ci) * 9 + dy * 3 + g, v);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // Fixed-order reduction of the per-CTA partial tiles of one wgrad_tc3 launch: element e = (grp * NTILE + col) * 128 + m of output tile
@@ -1241,33 +988,33 @@ __global__ void __launch_bounds__(256) wgrad3_finalize_kernel(const float* __res
   dw[((size_t)co * CinTot + ci_global + ci) * 9 + dy * 3 + g] += acc;
 }
 
-template <int CWB, int CWN, int NBOX>
+template <int CWB, int NTILE>
 int launch_wgrad3(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorMap& mx1, Wgrad3Params p, int n_tiles,
                   float* partial_ws, long long partial_floats, cudaStream_t stream) {
-  constexpr bool DYN = (NBOX == 1);
-  constexpr int per_stage = NBOX * TILE_M * CWN * 2 + 12 * 1024;
+  constexpr int per_stage = TILE_M * NTILE * 2 + 12 * 1024;
   constexpr int STAGES = per_stage >= 40 * 1024 ? 3 : 4;
-  using S = Wgrad3Smem<CWB, CWN, NBOX, STAGES, DYN>;
+  using S = Wgrad3Smem<CWB, NTILE, STAGES>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc3_kernel<CWB, CWN, NBOX, STAGES, DYN>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tc3_kernel<CWB, NTILE, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
     if (e != cudaSuccess) { wsl_set_error("wgrad_tc3: cudaFuncSetAttribute(%d bytes): %s", S::TOTAL, cudaGetErrorString(e)); return -5; }
     attr = true;
   }
   const int gy = n_tiles * (p.k_tiles0 + p.k_tiles1);
-  // narrow layers are bounded by the per-CTA rate of 32/64-byte TMA rows: two CTAs per SM (TMEM and smem allow it)
-  constexpr int per_sm = (DYN && CWN <= 32 && S::TOTAL <= 100 * 1024) ? 2 : 1;
-  int splits = (148 * per_sm + gy - 1) / gy;
+  int per_sm = 1;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wgrad_tc3_kernel<CWB, NTILE, STAGES>, NUM_THREADS, S::TOTAL);
+  if (per_sm < 1) per_sm = 1;
+  if (per_sm > 2) per_sm = 2;
+  int splits = (wsl_num_sms() * per_sm + gy - 1) / gy;
   if (splits > p.nchunks) splits = p.nchunks;
   if (splits < 1) splits = 1;
   dim3 grid(splits, gy);
-  constexpr int NTILE = CWN * NBOX;
   const long long need = (long long)splits * gy * 3 * NTILE * 128;
   p.partials = (partial_ws != nullptr && need <= partial_floats) ? partial_ws : nullptr;     // too small a workspace: atomics
-  wgrad_tc3_kernel<CWB, CWN, NBOX, STAGES, DYN><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
+  wgrad_tc3_kernel<CWB, NTILE, STAGES><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
   int rc = wsl_check_launch("wgrad_tc3");
   if (rc || p.partials == nullptr) return rc;
-  wgrad3_finalize_kernel<<<dim3((3 * NTILE * 128 + 255) / 256, gy), 256, 0, stream>>>(p.partials, splits, NTILE, CWB, DYN ? 1 : 0, p.k_tiles0,
+  wgrad3_finalize_kernel<<<dim3((3 * NTILE * 128 + 255) / 256, gy), 256, 0, stream>>>(p.partials, splits, NTILE, CWB, 1, p.k_tiles0,
                                                                                      p.k_tiles0 + p.k_tiles1, p.C0, p.C0 + p.C1, p.CoutReal, p.dw);
   return wsl_check_launch("wgrad3_finalize");
 }
@@ -1317,7 +1064,7 @@ int launch_wgrad(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorM
     attr = true;
   }
   const int gy = m_tiles * (p.n_tiles0 + p.n_tiles1) * p.tap_groups;
-  int splits = (148 * 2 + gy - 1) / gy;
+  int splits = (wsl_num_sms() * 2 + gy - 1) / gy;
   if (splits > p.nchunks) splits = p.nchunks;
   if (splits < 1) splits = 1;
   dim3 grid(splits, gy);
@@ -1441,17 +1188,15 @@ int launch_conv2(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap
     attr_bytes = smem;
   }
   const int n_tiles = p.CoutP / NT;
-  int occ = (220 * 1024) / smem;
-  const int occ_tmem = 512 / (int)Cfg::TMEM_COLS;
-  if (occ > occ_tmem) occ = occ_tmem;
-  if (occ > 4) occ = 4;
+  int occ = 1;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_tc2_kernel<KS, KBLK, NT, MT, STAGES>, NUM_THREADS, smem);
   if (occ < 1) occ = 1;
-  int gx = (148 * occ) / n_tiles;
+  int gx = (wsl_num_sms() * occ) / n_tiles;
   if (gx < 1) gx = 1;
   if (gx > p.ntiles) gx = p.ntiles;
   dim3 grid(gx, n_tiles);
   g_conv2_last_rows = gx;
-  conv_tc2_kernel<KS, KBLK, NT, MT, STAGES><<<grid, Conv2Epi<NT, MT>::THREADS, smem, stream>>>(a0, a1, b, p, w_bytes);
+  conv_tc2_kernel<KS, KBLK, NT, MT, STAGES><<<grid, NUM_THREADS, smem, stream>>>(a0, a1, b, p, w_bytes);
   return wsl_check_launch("conv_tc2");
 }
 
@@ -1460,54 +1205,44 @@ int conv2_dispatch_nt(int nt, const CUtensorMap& a0, const CUtensorMap& a1, cons
   switch (nt) {
     case 16:  return launch_conv2<KS, KBLK, 16, MT>(a0, a1, b, p, st);
     case 32:  return launch_conv2<KS, KBLK, 32, MT>(a0, a1, b, p, st);
-    case 64:  return launch_conv2<KS, KBLK, 64, MT>(a0, a1, b, p, st);
-    case 128: if constexpr (MT <= 2) return launch_conv2<KS, KBLK, 128, MT>(a0, a1, b, p, st); else break;
+    case 64:  if constexpr (MT <= 2) return launch_conv2<KS, KBLK, 64, MT>(a0, a1, b, p, st); else break;
+    case 128: if constexpr (MT == 1) return launch_conv2<KS, KBLK, 128, MT>(a0, a1, b, p, st); else break;
   }
   wsl_set_error("conv_tc2: unsupported N tile %d", nt);
   return -1;
 }
 
-
 // ================================================================================================
 // conv_row: 3x3 convolution for narrow outputs (CoutP = 16 or 32) with the filter ROWS in the MMA's N dimension.
 //
-// A tcgen05.mma (SS, M = 128, K = 16) costs ~43 + N/2 cycles on the B200 (profiles/micro/mma_rate.cu): the 4 KB A-operand
-// read dominates when N = Cout is 16 or 32, and conv_tc2's nine N = 16 MMAs per 128 pixels (459 cycles) bound the
-// full-resolution layers, not HBM.  Here the work unit is one INPUT row of 128 pixels:
+// With N = Cout = 16 or 32 an MMA is bound by reading its A operand, and conv_tc2 issues nine of them per 128 pixels.
+// Here the work unit is one INPUT row of 128 pixels:
 //     E_i[c][(dy, co)] = sum_{dx, ci} X[row i][c + dx - 1][ci] * W[dy][dx][co][ci]
-// i.e. 3 MMAs per 16 input channels (dx = pixel-shifted views of ONE row buffer), each with N = 3*Cout, accumulated into a
-// ring slot of 3*Cout TMEM columns; an output row is then
+// i.e. 3 MMAs per 16 input channels (dx = pixel-shifted views of ONE row buffer), each with N = 3*Cout; an output row is
 //     out[r][c] = E_r[c][dy=0] + E_{r+1}[c][dy=1] + E_{r+2}[c][dy=2]
-// -- three column groups of three ring slots in the SAME TMEM lane, summed by the epilogue thread that owns pixel c: no
-// cross-lane traffic.  201 cycles per 128 pixels for 16 -> 16 channels instead of 459.
-//   warp 0: TMA producer (one [16 ch x 130 px] box per input row and 16-channel block; OOB zero fill = padding)
-//   warp 1: MMA issuer;  warps 2..5: epilogue (lane = pixel; 1 KB contiguous bf16 per warp and output row).
+// summed in registers by the thread that owns pixel c (a rolling pair of partial rows): no cross-thread traffic.
+//   warp 8: TMA producer (one [KBW ch x 130 px] box per input row and channel block; OOB zero fill = padding)
+//   warpgroup h: pixels 64h .. 64h+63 of the strip (MMA issue + epilogue).
 // Work item = (image, 128-pixel column strip, segment of RS output rows); persistent CTAs walk the items.
 // ================================================================================================
 constexpr int ROW_PX = 128;
 // bytes of one input-row buffer: 130 halo pixels x KBW channels, padded to a multiple of the 8-row swizzle atom
 __host__ __device__ constexpr int row_abytes(int kbw) { return ((130 * kbw * 2 + 255) / 256) * 256; }
 
-template <int NT, int RING, int EW, int KBW>
-__global__ void __launch_bounds__(64 + 32 * EW, (RING * 3 * NT <= 256) ? 2 : 1) conv_row_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
-                                                       const __grid_constant__ CUtensorMap map_b, const ConvV2Params p, const int KB,
-                                                       const int RS, const int w_bytes, const int STAGES) {
+template <int NT, int KBW>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
+                                                                  const __grid_constant__ CUtensorMap map_b, const ConvV2Params p, const int KB,
+                                                                  const int RS, const int w_bytes, const int STAGES) {
   constexpr int NG = 3 * NT;                              // accumulator columns of one input row (three filter rows)
   constexpr int SWB = KBW * 2, ROW_ABYTES = row_abytes(KBW);   // channel block = swizzle span: 32 B (16 ch) or 64 B (32 ch)
-  // (a 64-byte block halves the number of TMA rows per box: the producer is bounded by ~5 cycles per TMA row and CTA)
-  constexpr uint32_t TMEM_COLS = (RING * NG <= 256) ? 256 : 512;
-  static_assert(RING * NG <= 512 && RING >= 4, "TMEM ring");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* w_smem = smem;                                 // [KB][dx][3*NT rows x 32 B]
+  uint8_t* w_smem = smem;                                 // [KB][dx][3*NT rows x SWB]
   uint8_t* a_smem = smem + w_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + (size_t)STAGES * KB * ROW_ABYTES);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + STAGES;
-  uint64_t* e_full = bars + 2 * STAGES;
-  uint64_t* e_empty = e_full + RING;
-  uint64_t* w_bar = e_empty + RING;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_bar + 1);
+  uint64_t* w_bar = bars + 2 * STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kb0 = p.C0 / KBW;
@@ -1517,20 +1252,17 @@ __global__ void __launch_bounds__(64 + 32 * EW, (RING * 3 * NT <= 256) ? 2 : 1) 
   const int rows_in = RS + 2;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < RING; ++s) { mbar_init(&e_full[s], 1); mbar_init(&e_empty[s], 4); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], CONSUMER_WARPS); }
     mbar_init(w_bar, 1);
     fence_barrier_init();
     prefetch_tmap(&map_a0);
     prefetch_tmap(&map_b);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= PRODUCER_WARP) {
+    producer_regs();
+    if (warp != PRODUCER_WARP) return;
     if (lane == 0) {
       mbar_expect_tx(w_bar, (uint32_t)(KB * 9 * NT * SWB));
       for (int kb = 0; kb < KB; ++kb)
@@ -1539,8 +1271,7 @@ __global__ void __launch_bounds__(64 + 32 * EW, (RING * 3 * NT <= 256) ? 2 : 1) 
             tma_load_3d(&map_b, w_bar, w_smem + (((kb * 3 + dx) * 3 + dy) * NT) * SWB, kb * KBW, 0, dy * 3 + dx);
     }
     __syncwarp();
-    // row loop: the warp stays converged, one elected lane issues with warp-uniform operands (a divergent lane-0 branch
-    // costs a few hundred cycles per TMA instruction, and this kernel issues one or two per 128 pixels)
+    // row loop: the warp stays converged, one elected lane issues with warp-uniform operands
     const uint32_t elected = elect_one();
     const uint32_t a_u = uniform(smem_u32(a_smem)), full_u = uniform(smem_u32(a_full));
     int s = 0;
@@ -1568,183 +1299,112 @@ __global__ void __launch_bounds__(64 + 32 * EW, (RING * 3 * NT <= 256) ? 2 : 1) 
         if (++s == STAGES) { s = 0; sph ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = idesc_for(make_idesc_bf16(NG), p.dt);
-    constexpr uint32_t d_hi = desc_hi<SWB>(8 * SWB);
-    const uint32_t elected = elect_one();
-    const uint32_t tmem_u = uniform(tmem_base);
-    const uint32_t a_lo0 = (uniform(smem_u32(a_smem)) >> 4) | 0x10000u;
-    const uint32_t w_lo0 = (uniform(smem_u32(w_smem)) >> 4) | 0x10000u;
-    mbar_wait(w_bar, 0);
-    const int total_rows = my_items * rows_in;
-    int s = 0, slot = 0;
-    uint32_t sph = 0, rph = 1;           // parities: a_full[s] (first completion), e_empty[slot] (fresh barrier passes)
-    for (int q = 0; q < total_rows; ++q) {
-      mbar_wait(&e_empty[slot], rph);
+    return;
+  }
+  consumer_regs();
+  // consumers: bias from shared memory, BatchNorm partial sums accumulated per thread and combined once at the end
+  __shared__ float s_bias[NT];
+  const int h = threadIdx.x >> 7, t = threadIdx.x & 127;
+  if (threadIdx.x < NT) s_bias[threadIdx.x] = p.bias ? p.bias[threadIdx.x] : 0.f;
+  asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+  const uint32_t a_u = smem_u32(a_smem) + (uint32_t)(64 * h * SWB), w_u = smem_u32(w_smem);
+  float ls[NT / 4], lq[NT / 4];
+#pragma unroll
+  for (int k = 0; k < NT / 4; ++k) ls[k] = lq[k] = 0.f;
+  mbar_wait(w_bar, 0);
+  int s = 0;
+  uint32_t sph = 0;
+  for (int it = 0; it < my_items; ++it) {
+    const int item = blockIdx.x + it * gridDim.x;
+    const int seg = item % segs, t1 = item / segs, strip = t1 % strips, n = t1 / strips;
+    const int y0 = seg * RS;
+    float pa[NT / 2], pb[NT / 2];       // partial output rows i-2 (dy 0 + 1 summed) and i-1 (dy 0)
+#pragma unroll
+    for (int e = 0; e < NT / 2; ++e) pa[e] = pb[e] = 0.f;
+    for (int i = 0; i < rows_in; ++i) {
+      float acc[NG / 2];
+#pragma unroll
+      for (int e = 0; e < NG / 2; ++e) acc[e] = 0.f;
       mbar_wait(&a_full[s], sph);
-      tc_fence_after();
-      if (elected) {
-        const uint32_t d = tmem_u + (uint32_t)(slot * NG);
-        for (int kb = 0; kb < KB; ++kb) {
-          const uint32_t a_lo = a_lo0 + (uint32_t)((s * KB + kb) * (ROW_ABYTES >> 4));
-          const uint32_t w_lo = w_lo0 + (uint32_t)(kb * 3 * ((NG * SWB) >> 4));
+      wgmma_fence();
+      for (int kb = 0; kb < KB; ++kb) {
+        const uint32_t a_lo = a_u + (uint32_t)((s * KB + kb) * ROW_ABYTES);
+        const uint32_t w_lo = w_u + (uint32_t)(kb * 3 * NG * SWB);
 #pragma unroll
-          for (int ks = 0; ks < KBW / 16; ++ks) {
+        for (int ks = 0; ks < KBW / 16; ++ks) {
 #pragma unroll
-            for (int dx = 0; dx < 3; ++dx)
-              umma_f16_w(d, a_lo + (uint32_t)(dx * (SWB >> 4) + ks * 2), d_hi, w_lo + (uint32_t)(dx * ((NG * SWB) >> 4) + ks * 2), d_hi, idesc,
-                         (kb > 0 || ks > 0 || dx > 0) ? 1u : 0u);
-          }
+          for (int dx = 0; dx < 3; ++dx)
+            Wgmma<NG>::template mma<0, 0>(acc, gmma_desc<SWB>(a_lo + (uint32_t)(dx * SWB + 32 * ks), 16, 8 * SWB),
+                                          gmma_desc<SWB>(w_lo + (uint32_t)(dx * NG * SWB + 32 * ks), 16, 8 * SWB),
+                                          (kb > 0 || ks > 0 || dx > 0) ? 1u : 0u, p.dt);
         }
-        umma_commit(&a_empty[s]);
-        umma_commit(&e_full[slot]);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>();
+      release_stage(&a_empty[s]);
       if (++s == STAGES) { s = 0; sph ^= 1u; }
-      if (++slot == RING) { slot = 0; rph ^= 1u; }
-    }
-  } else {
-    // EW epilogue warps: warp%4 selects the TMEM lane quarter (= 32-pixel group of the strip), (warp-2)/4 the set of output
-    // rows (j % SETS) it owns.  The per-128-pixel MMA time is short here, so the epilogue must be cheap: bias from shared
-    // memory, BatchNorm partial sums accumulated per lane (pixel) and transposed once at the end.
-    constexpr int SETS = EW / 4;
-    __shared__ float s_bias[NT];
-    __shared__ float s_stat[EW][2][NT];
-    const int ew = warp - 2, qt = warp & 3, set = ew >> 2;
-    if (ew == 0 && lane < NT) s_bias[lane] = p.bias ? p.bias[lane] : 0.f;
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
-    const uint32_t lane_base = tmem_base + ((uint32_t)(qt * 32) << 16);
-    float ls[NT], lq[NT];
+      wgmma_fence_regs(acc);
+      // column 8*j + frag_col + b of E: filter row j / (NT/8), output channel 8*(j % (NT/8)) + frag_col + b
+      if (i >= 2) {                                   // output row i - 2 is complete
+        const int gy = y0 + i - 2;
 #pragma unroll
-    for (int c = 0; c < NT; ++c) ls[c] = lq[c] = 0.f;
-    int q0 = 0;
-    for (int it = 0; it < my_items; ++it, q0 += rows_in) {
-      const int item = blockIdx.x + it * gridDim.x;
-      const int seg = item % segs, t1 = item / segs, strip = t1 % strips, n = t1 / strips;
-      const int y0 = seg * RS, gx = strip * ROW_PX + qt * 32 + lane;
-      for (int j = set; j < RS; j += SETS) {
-        const int qa = q0 + j, qb = qa + 1, qc = qa + 2;
-        mbar_wait(&e_full[qc % RING], (qc / RING) & 1);    // commits complete in order: rows qa, qb are done as well
-        tc_fence_after();
-        const int gy = y0 + j;
+        for (int ii = 0; ii < 2; ++ii) {
+          const int gx = strip * ROW_PX + 64 * h + frag_row(t) + 8 * ii;
 #pragma unroll
-        for (int c = 0; c < NT; c += 16) {
-          float v[16], u1[16], u2[16];
-          tmem_ld16_nowait(lane_base + (uint32_t)((qa % RING) * NG + 0 * NT + c), v);
-          tmem_ld16_nowait(lane_base + (uint32_t)((qb % RING) * NG + 1 * NT + c), u1);
-          tmem_ld16_nowait(lane_base + (uint32_t)((qc % RING) * NG + 2 * NT + c), u2);
-          tmem_ld_wait();
-          if (c + 16 >= NT) {                               // all reads of this output row are done: release ring slots
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              mbar_arrive(&e_empty[qa % RING]);
-              if (j == RS - 1) { mbar_arrive(&e_empty[qb % RING]); mbar_arrive(&e_empty[qc % RING]); }
+          for (int jj = 0; jj < NT / 8; ++jj) {
+            const int c = 8 * jj + frag_col(t), e = 4 * jj + 2 * ii;
+            const float v0 = (pa[e] + acc[4 * (2 * NT / 8 + jj) + 2 * ii]) + s_bias[c];
+            const float v1 = (pa[e + 1] + acc[4 * (2 * NT / 8 + jj) + 2 * ii + 1]) + s_bias[c + 1];
+            if (p.out_mode == 0 && p.stat_partials) {   // statistics of the values exactly as stored (rounded to the 16-bit type)
+              float2 r;
+              if (p.dt == 2) r = __half22float2(__floats2half2_rn(v0, v1));
+              else r = __bfloat1622float2(__floats2bfloat162_rn(v0, v1));
+              ls[2 * jj] += r.x;     lq[2 * jj] = fmaf(r.x, r.x, lq[2 * jj]);
+              ls[2 * jj + 1] += r.y; lq[2 * jj + 1] = fmaf(r.y, r.y, lq[2 * jj + 1]);
             }
-          }
-#pragma unroll
-          for (int jj = 0; jj < 16; jj += 4) {
-            const float4 bb = *reinterpret_cast<const float4*>(&s_bias[c + jj]);
-            v[jj + 0] = ((v[jj + 0] + u1[jj + 0]) + u2[jj + 0]) + bb.x;
-            v[jj + 1] = ((v[jj + 1] + u1[jj + 1]) + u2[jj + 1]) + bb.y;
-            v[jj + 2] = ((v[jj + 2] + u1[jj + 2]) + u2[jj + 2]) + bb.z;
-            v[jj + 3] = ((v[jj + 3] + u1[jj + 3]) + u2[jj + 3]) + bb.w;
-          }
-          if (p.out_mode == 0) {
-            float lo[8], hi[8];
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) { lo[jj] = v[jj]; hi[jj] = v[8 + jj]; }
-            const uint4 plo = pack8_dt(lo, p.dt), phi = pack8_dt(hi, p.dt);
-            if (c < p.CoutStore) {
-              __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + (((long long)n * p.H + gy) * p.W + gx) * p.CoutStore + c;
-              reinterpret_cast<uint4*>(o)[0] = plo;
-              if (c + 8 < p.CoutStore) reinterpret_cast<uint4*>(o)[1] = phi;
-            }
-            if (p.stat_partials) {   // statistics of the values exactly as stored (rounded to the 16-bit type)
-              unpack8_dt(plo, lo, p.dt);
-              unpack8_dt(phi, hi, p.dt);
-#pragma unroll
-              for (int jj = 0; jj < 8; ++jj) {
-                ls[c + jj] += lo[jj];           lq[c + jj] = fmaf(lo[jj], lo[jj], lq[c + jj]);
-                ls[c + 8 + jj] += hi[jj];       lq[c + 8 + jj] = fmaf(hi[jj], hi[jj], lq[c + 8 + jj]);
-              }
-            }
-          } else {
-            float* o = reinterpret_cast<float*>(p.out);
-#pragma unroll
-            for (int jj = 0; jj < 16; ++jj)
-              if (c + jj < p.CoutStore) o[(((long long)n * p.CoutStore + c + jj) * p.H + gy) * p.W + gx] = v[jj];
+            store_pair(p.out, p.out_mode == 0 ? 0 : 1, p.dt, p.CoutStore, p.H, p.W, n, gy, gx, c, v0, v1);
           }
         }
       }
-      // every set must have released its rows before the ring indices of the next item are reused: nothing to do, the
-      // e_empty arrivals above are per row and each row is owned by exactly one set
-    }
-    if (p.stat_partials) {
 #pragma unroll
-      for (int c = 0; c < NT; c += 16) {
-        float a[16], b[16];
+      for (int ii = 0; ii < 2; ++ii)
 #pragma unroll
-        for (int jj = 0; jj < 16; ++jj) { a[jj] = ls[c + jj]; b[jj] = lq[c + jj]; }
-        const float sa = warp_transpose_sum16(a, lane), sb = warp_transpose_sum16(b, lane);
-        if ((lane & 1) == 0) {
-          s_stat[ew][0][c + ((lane >> 1) & 15)] = sa;
-          s_stat[ew][1][c + ((lane >> 1) & 15)] = sb;
-        }
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
-      const int t = threadIdx.x - 64;
-      for (int c = t; c < 2 * NT; c += 32 * EW) {
-        const int which = c / NT, ch = c % NT;
-        float a = 0.f;
+        for (int jj = 0; jj < NT / 8; ++jj)
 #pragma unroll
-        for (int w = 0; w < EW; ++w) a += s_stat[w][which][ch];
-        p.stat_partials[((size_t)blockIdx.x * 2 + which) * p.CoutP + ch] = a;
-      }
+          for (int b = 0; b < 2; ++b) {
+            const int e = 4 * jj + 2 * ii + b;
+            pa[e] = pb[e] + acc[4 * (NT / 8 + jj) + 2 * ii + b];   // output row i - 1: + filter row 1
+            pb[e] = acc[4 * jj + 2 * ii + b];                       // output row i: filter row 0
+          }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
+  if (p.out_mode == 0 && p.stat_partials) write_stat_partials<NT>(ls, lq, p.stat_partials, p.CoutP, 0);
 }
 
-template <int NT, int RING, int EW, int KBW>
-int launch_conv_row_cfg(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, int KB, int RS,
-                        int STAGES, cudaStream_t stream) {
+template <int NT, int KBW>
+int launch_conv_row(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, int KB, int RS,
+                    cudaStream_t stream) {
+  // Row buffers in flight: ~80 KB per SM cover the HBM latency.
+  static const int st_env = [] { const char* e = getenv("WSL4MIS_ROW_STAGES"); return e ? atoi(e) : 0; }();
+  const int STAGES = st_env ? st_env : (KB == 1 ? 12 : KB == 2 ? 8 : 6);
   const int w_bytes = ((KB * 9 * NT * KBW * 2 + 1023) / 1024) * 1024;
   const int smem = w_bytes + STAGES * KB * row_abytes(KBW) + 1024 + 256;
   if (smem > 220 * 1024) { wsl_set_error("conv_row: %d bytes of shared memory needed", smem); return -6; }
   static int attr_bytes = 0;
   if (smem > attr_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(conv_row_kernel<NT, RING, EW, KBW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_row_kernel<NT, KBW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { wsl_set_error("conv_row: cudaFuncSetAttribute(%d): %s", smem, cudaGetErrorString(e)); return -5; }
     attr_bytes = smem;
   }
   const int items = p.N * (p.W / ROW_PX) * (p.H / RS);
-  int occ = (RING * 3 * NT <= 256) ? 2 : 1;
-  if ((220 * 1024) / smem < occ) occ = 1;
-  int gx = 148 * occ;
+  int occ = 1;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_row_kernel<NT, KBW>, NUM_THREADS, smem);
+  if (occ < 1) occ = 1;
+  int gx = wsl_num_sms() * occ;
   if (gx > items) gx = items;
   g_conv2_last_rows = gx;
-  conv_row_kernel<NT, RING, EW, KBW><<<gx, 64 + 32 * EW, smem, stream>>>(a0, a1, b, p, KB, RS, w_bytes, STAGES);
+  conv_row_kernel<NT, KBW><<<gx, NUM_THREADS, smem, stream>>>(a0, a1, b, p, KB, RS, w_bytes, STAGES);
   return wsl_check_launch("conv_row");
-}
-
-template <int NT>
-int launch_conv_row(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, int KB, int RS, int kbw,
-                    cudaStream_t stream) {
-  // NT = 16: either one CTA per SM owning the whole TMEM (ring of 10 row accumulators, 12 epilogue warps) or two CTAs with
-  // half of it each (ring of 5, 8 epilogue warps); NT = 32: one CTA (ring of 5 x 96 columns), 8 epilogue warps.
-  // KB counts channel blocks of kbw channels.  Row buffers in flight: ~80 KB per SM cover the HBM latency.
-  static const int cfg = [] { const char* e = getenv("WSL4MIS_ROW_CFG"); return e ? atoi(e) : 1; }();
-  static const int st_env = [] { const char* e = getenv("WSL4MIS_ROW_STAGES"); return e ? atoi(e) : 0; }();
-  if constexpr (NT == 16) {
-    if (cfg == 1 && KB <= 2) return launch_conv_row_cfg<16, 5, 8, 16>(a0, a1, b, p, KB, RS, st_env ? st_env : (KB == 1 ? 10 : 6), stream);
-    return launch_conv_row_cfg<16, 10, 12, 16>(a0, a1, b, p, KB, RS, st_env ? st_env : (KB <= 2 ? 12 : 8), stream);
-  } else {
-    if (kbw == 32) return launch_conv_row_cfg<32, 5, 8, 32>(a0, a1, b, p, KB, RS, st_env ? st_env : (KB == 1 ? 12 : 8), stream);
-    return launch_conv_row_cfg<32, 5, 8, 16>(a0, a1, b, p, KB, RS, st_env ? st_env : (KB == 1 ? 16 : KB == 2 ? 12 : 8), stream);
-  }
 }
 
 }  // namespace
@@ -1824,7 +1484,7 @@ static int wgrad_tc_impl(const void* src0, int C0, const void* src1, int C1, con
   WSL_REQUIRE(W % TILE_W == 0 && H % TILE_H == 0, "wsl_wgrad_tc: H,W must be multiples of the 8x16 pixel tile (got %dx%d)", H, W);
   const int cwa = CoutP >= 64 ? 64 : CoutP;       // 16 / 32 / 64
   WSL_REQUIRE(cwa == 16 || cwa == 32 || cwa == 64, "wsl_wgrad_tc: unsupported CoutP %d", CoutP);
-  WSL_REQUIRE(CoutP < 128 || CoutP % 64 == 0, "wsl_wgrad_tc: CoutP >= 128 must be a multiple of 64");   // a half-filled last tile reads zeros (TMA)
+  WSL_REQUIRE(CoutP <= 64 || CoutP % 64 == 0, "wsl_wgrad_tc: CoutP above 64 must be a multiple of 64 (got %d)", CoutP);   // one dY box per 64 couts
   int cwb = 64;
   while (cwb > 16 && (C0 % cwb != 0 || (C1 > 0 && C1 % cwb != 0))) cwb >>= 1;
   const int na = CoutP >= 128 ? 2 : 1;
@@ -1941,7 +1601,7 @@ WSL_API int wsl_channel_sum(const void* x, int dtype, long long P, int C, int Cr
   WSL_REQUIRE(C % 8 == 0 && C / 8 <= 256 && Creal <= C, "wsl_channel_sum: unsupported channel count %d", C);
   const int rows = 256 / (C / 8);
   long long b = (P + rows * 16 - 1) / (rows * 16);
-  if (b > 148 * 2) b = 148 * 2;
+  if (b > wsl_num_sms() * 2) b = wsl_num_sms() * 2;
   if (b < 1) b = 1;
   if (dtype == 1) channel_sum_kernel<float><<<(int)b, 256, 256 * 8 * sizeof(float), stream>>>((const float*)x, P, C, Creal, out, ws);
   else if (dtype == 2) channel_sum_kernel<__nv_bfloat16, true><<<(int)b, 256, 256 * 8 * sizeof(float), stream>>>((const __nv_bfloat16*)x, P, C, Creal, out, ws);
@@ -1964,7 +1624,7 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
     const int kbw = (wide_on && CoutP == 32 && C0 % 32 == 0 && C1 % 32 == 0) ? 32 : 16;
     const int KB = (C0 + C1) / kbw;
     // row segments of 32 output rows (6 % halo re-reads) unless that leaves fewer than ~4 work items per SM
-    const int RS = (H % 32 == 0 && (long long)N * (W / ROW_PX) * (H / 32) >= 4 * 148) ? 32 : 16;
+    const int RS = (H % 32 == 0 && (long long)N * (W / ROW_PX) * (H / 32) >= 4 * wsl_num_sms()) ? 32 : 16;
     if (row_on && ksize == 3 && (CoutP == 16 || CoutP == 32) && W % ROW_PX == 0 && H % 16 == 0 && (C0 + C1) <= 64) {
       CUtensorMap a0, a1, b;
       {
@@ -1990,10 +1650,11 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
       ConvV2Params p;
       p.N = N; p.H = H; p.W = W; p.C0 = C0; p.C1 = C1; p.CoutP = CoutP; p.CoutStore = CoutStore;
       p.tiles_x = 0; p.tiles_y = 0; p.ntiles = 0;
-      p.out_mode = out_mode; p.desc_mode = 0; p.dt = dtype; p.bias = bias; p.out = out;
+      p.out_mode = out_mode; p.dt = dtype; p.bias = bias; p.out = out;
       p.stat_partials = (out_mode == 0) ? stat_partials : nullptr;
-      const int rc = (CoutP == 16) ? launch_conv_row<16>(a0, a1, b, p, KB, RS, kbw, stream)
-                                   : launch_conv_row<32>(a0, a1, b, p, KB, RS, kbw, stream);
+      const int rc = (CoutP == 16) ? launch_conv_row<16, 16>(a0, a1, b, p, KB, RS, stream)
+                     : (kbw == 32)   ? launch_conv_row<32, 32>(a0, a1, b, p, KB, RS, stream)
+                                     : launch_conv_row<32, 16>(a0, a1, b, p, KB, RS, stream);
       if (stat_rows_host) *stat_rows_host = g_conv2_last_rows;
       return rc;
     }
@@ -2004,13 +1665,11 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
   while (mt > 1 && H % (16 * mt) != 0) mt >>= 1;
   WSL_REQUIRE(W % 8 == 0 && H % (16 * mt) == 0, "wsl_conv_tc2: H,W must be multiples of the 16x8 pixel tile (got %dx%d)", H, W);
   const int CinP = C0 + C1, T = ksize * ksize;
-  // N tile: largest of 128/64/32/16 dividing CoutP whose resident weight slice fits (~148 KB) and TMEM (2*MT*NT <= 512)
+  // N tile: largest of 128/64/32/16 dividing CoutP whose resident weight slice fits (~148 KB) and whose accumulators
+  // fit the registers (MT*NT <= 128: 64 fp32 per consumer thread)
   int nt = CoutP >= 128 ? 128 : CoutP;
-  while (nt > 16 && (CoutP % nt != 0 || (long long)T * CinP * nt * 2 > 148 * 1024 || 2 * mt * nt > 512 || (nt == 128 && mt > 2))) nt >>= 1;
+  while (nt > 16 && (CoutP % nt != 0 || (long long)T * CinP * nt * 2 > 148 * 1024 || mt * nt > 128)) nt >>= 1;
   WSL_REQUIRE(CoutP % nt == 0 && (long long)T * CinP * nt * 2 <= 152 * 1024, "wsl_conv_tc2: weights do not fit (Cin %d, NT %d)", CinP, nt);
-  // base_offset stays 0: the swizzle XOR is taken from absolute shared-memory address bits by both TMA and tcgen05
-  // (verified on B200: setting base_offset = (addr>>7)&7 for the row-shifted views breaks every case).
-  const int desc_mode = 0;
   const int pad = ksize / 2;
   CUtensorMap a0, a1, b;
   {
@@ -2036,7 +1695,7 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
   ConvV2Params p;
   p.N = N; p.H = H; p.W = W; p.C0 = C0; p.C1 = C1; p.CoutP = CoutP; p.CoutStore = CoutStore;
   p.tiles_x = W / 8; p.tiles_y = H / (16 * mt); p.ntiles = N * p.tiles_x * p.tiles_y;
-  p.out_mode = out_mode; p.desc_mode = desc_mode; p.dt = dtype; p.bias = bias; p.out = out;
+  p.out_mode = out_mode; p.dt = dtype; p.bias = bias; p.out = out;
   p.stat_partials = (out_mode == 0) ? stat_partials : nullptr;
 #define WSL_C2(KS_, KB_, MT_)                                                   \
   do {                                                                         \
@@ -2069,7 +1728,7 @@ WSL_API int wsl_wgrad_tc2(const void* src0, int C0, const void* src1, int C1, co
   WSL_REQUIRE(CoutP % 16 == 0 && (CoutP < 128 || CoutP % 128 == 0), "wsl_wgrad_tc2: unsupported CoutP %d", CoutP);
   WSL_REQUIRE(W % 8 == 0 && H % 16 == 0, "wsl_wgrad_tc2: H,W must be multiples of the 16x8 pixel chunk (got %dx%d)", H, W);
   const int cwa = CoutP >= 64 ? 64 : CoutP;
-  const int cwb = (C0 % 32 == 0 && (C1 == 0 || C1 % 32 == 0)) ? 32 : 16;
+  const int cwb = 16;          // nine accumulators of CWB/2 registers per consumer thread: 16-channel blocks keep them in registers
   const int na = CoutP >= 128 ? 2 : 1;
   const int m_tiles = CoutP >= 128 ? CoutP / 128 : 1;
   CUtensorMap mdy, mx0, mx1;
@@ -2097,12 +1756,6 @@ WSL_API int wsl_wgrad_tc2(const void* src0, int C0, const void* src1, int C1, co
   p.N = N; p.H = H; p.W = W; p.C0 = C0; p.C1 = C1; p.CoutP = CoutP; p.CoutReal = CoutReal; p.taps = 9; p.ks = 3;
   p.tiles_x = W / 8; p.tiles_y = H / 16; p.nchunks = N * p.tiles_x * p.tiles_y;
   p.n_tiles0 = C0 / cwb; p.n_tiles1 = C1 / cwb; p.tap_groups = 1; p.dt = dtype; p.scale_a = nullptr; p.scale_b = nullptr; p.dw = dw; p.partials = nullptr; p.dil = 1;
-  if (cwb == 32) {
-    if (cwa == 64 && na == 2) return launch_wgrad2<64, 2, 32>(mdy, mx0, mx1, p, m_tiles, stream);
-    if (cwa == 64) return launch_wgrad2<64, 1, 32>(mdy, mx0, mx1, p, m_tiles, stream);
-    if (cwa == 32) return launch_wgrad2<32, 1, 32>(mdy, mx0, mx1, p, m_tiles, stream);
-    return launch_wgrad2<16, 1, 32>(mdy, mx0, mx1, p, m_tiles, stream);
-  }
   if (cwa == 64 && na == 2) return launch_wgrad2<64, 2, 16>(mdy, mx0, mx1, p, m_tiles, stream);
   if (cwa == 64) return launch_wgrad2<64, 1, 16>(mdy, mx0, mx1, p, m_tiles, stream);
   if (cwa == 32) return launch_wgrad2<32, 1, 16>(mdy, mx0, mx1, p, m_tiles, stream);
@@ -2120,25 +1773,24 @@ WSL_API int wsl_wgrad_tc3(const void* src0, int C0, const void* src1, int C1, co
   WSL_REQUIRE(W % 8 == 0 && H % 16 == 0, "wsl_wgrad_tc3: H,W must be multiples of the 16x8 pixel chunk (got %dx%d)", H, W);
   const int cwb = (C0 % 32 == 0 && (C1 == 0 || C1 % 32 == 0)) ? 32 : 16;
   const int cwn = CoutP >= 64 ? 64 : CoutP;
-  const int ntile = CoutP >= 128 ? 128 : CoutP;
+  const int ntile = CoutP >= 64 ? 64 : CoutP;     // N = 3*ntile <= 192 accumulator columns per consumer thread pair
   const int n_tiles = CoutP / ntile;
-  const bool dyn = ntile < 128;          // single dY box: filter rows merged into the MMA's N dimension (18-row dY box, 16-row X box)
   CUtensorMap mdy, mx0, mx1;
   {
     long long d[4] = {CoutP, W, H, N};
-    int bx[4] = {cwn, 8, dyn ? 18 : 16, 1};
+    int bx[4] = {cwn, 8, 18, 1};         // one halo row above and below: filter rows in the MMA's N dimension
     int rc = get_map(dy, 4, d, bx, cwn, &mdy, dtype);
     if (rc) return rc;
   }
   {
     long long d[4] = {C0, W, H, N};
-    int bx[4] = {cwb, 10, dyn ? 16 : 18, 1};
+    int bx[4] = {cwb, 10, 16, 1};
     int rc = get_map(src0, 4, d, bx, cwb, &mx0, dtype);
     if (rc) return rc;
   }
   if (C1 > 0) {
     long long d[4] = {C1, W, H, N};
-    int bx[4] = {cwb, 10, dyn ? 16 : 18, 1};
+    int bx[4] = {cwb, 10, 16, 1};
     int rc = get_map(src1, 4, d, bx, cwb, &mx1, dtype);
     if (rc) return rc;
   } else {
@@ -2149,10 +1801,9 @@ WSL_API int wsl_wgrad_tc3(const void* src0, int C0, const void* src1, int C1, co
   p.tiles_x = W / 8; p.tiles_y = H / 16; p.nchunks = N * p.tiles_x * p.tiles_y;
   p.k_tiles0 = C0 / cwb; p.k_tiles1 = C1 / cwb; p.dt = dtype; p.dw = dw; p.partials = nullptr;
 #define WSL_W3(CWB_) \
-  if (ntile == 128) return launch_wgrad3<CWB_, 64, 2>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream); \
-  if (ntile == 64) return launch_wgrad3<CWB_, 64, 1>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);  \
-  if (ntile == 32) return launch_wgrad3<CWB_, 32, 1>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);  \
-  return launch_wgrad3<CWB_, 16, 1>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);
+  if (ntile == 64) return launch_wgrad3<CWB_, 64>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);  \
+  if (ntile == 32) return launch_wgrad3<CWB_, 32>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);  \
+  return launch_wgrad3<CWB_, 16>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);
   if (cwb == 32) { WSL_W3(32) }
   WSL_W3(16)
 #undef WSL_W3

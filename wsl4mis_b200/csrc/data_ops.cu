@@ -81,7 +81,7 @@ WSL_API int wsl_augment_batch(const float* images, const uint8_t* labels, const 
   WSL_REQUIRE(B > 0 && OH > 0 && OW > 0, "wsl_augment_batch: empty batch or output (B=%d, %dx%d)", B, OH, OW);
   const long long total = (long long)B * OH * OW;
   long long blocks = (total + TPB * 4 - 1) / (TPB * 4);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > wsl_num_sms() * 8) blocks = wsl_num_sms() * 8;
   augment_batch_kernel<<<(int)blocks, TPB, 0, stream>>>(images, labels, reinterpret_cast<const AugSample*>(table), B, OH, OW, out_img,
                                                         out_lab);
   return wsl_check_launch("augment_batch");

@@ -884,7 +884,7 @@ __global__ void __launch_bounds__(TPB) nearest_resize_bwd_kernel(const float* __
 inline int grid_for(long long work_items, int per_block) {
   long long b = (work_items + per_block - 1) / per_block;
   if (b < 1) b = 1;
-  if (b > 148 * 8) b = 148 * 8;   // multiple of the SM count; grid-stride loops cover the rest
+  if (b > wsl_num_sms() * 8) b = wsl_num_sms() * 8;   // multiple of the SM count; grid-stride loops cover the rest
   return (int)b;
 }
 
@@ -924,7 +924,7 @@ WSL_API int wsl_gatedcrf_fwd(const float* probs, const float* image, float* gpro
   constexpr int TW = 32, TH = RT * WARPS;
   const int tx = (W + TW - 1) / TW, ty = (H + TH - 1) / TH;
   const long long ntiles = (long long)N * tx * ty;
-  int grid = (int)(ntiles < WSL_MAX_PARTIAL_BLOCKS ? ntiles : 148 * 12);
+  int grid = (int)(ntiles < WSL_MAX_PARTIAL_BLOCKS ? ntiles : wsl_num_sms() * 12);
   const size_t smem = (((TH + 2 * R) * (TW + 2 * R) + 3) & ~3) * sizeof(float) + (size_t)(TH + 2 * R) * (TW + 2 * R) * sizeof(float4);
   static bool attr_set = false;
   if (!attr_set) {

@@ -1,6 +1,6 @@
 // Network operators for the U-Net hot path on channels-last (NHWC) bf16 activations:
 //   * direct (CUDA-core) convolution forward / data-gradient / weight-gradient -- used for the layers that do
-//     not map to tcgen05 tiles (Cin = 1, tiny problems) and as the on-device cross-check of conv_tc.cu;
+//     not map to wgmma tiles (Cin = 1, tiny problems) and as the on-device cross-check of conv_tc.cu;
 //   * training-mode BatchNorm statistics, normalise + LeakyReLU + dropout (+ fused 2x2 max-pool), and the
 //     matching backward (reference: networks/unet.py:18-26,38);
 //   * bilinear x2 upsample (align_corners=True, networks/unet.py:56-57) forward / backward;
@@ -1278,11 +1278,11 @@ __global__ void __launch_bounds__(TPB) nhwc_bf16_to_nchw_f32_kernel(const T* __r
 // ================================================================================================
 // w: fp32 [Cout][Cin][KS][KS] (torch layout).  Outputs (any may be null):
 //   wf  fp32 [T][CinP][CoutP]      forward operand of conv_direct
-//   bf  bf16 [T][CoutP][CinP]      tcgen05 B operand, forward  (K-major: Cin contiguous)
+//   bf  bf16 [T][CoutP][CinP]      wgmma B operand, forward  (K-major: Cin contiguous)
 // and, for the input-channel slice [ci_begin, ci_begin+ci_count) (one slice per concatenated source), SliceP =
 // ci_count rounded up to 16:
 //   wd  fp32 [T][CoutP][SliceP]    dgrad operand of conv_direct (tap flipped, roles swapped)
-//   bd  bf16 [T][SliceP][CoutP]    tcgen05 B operand, dgrad    (K-major: Cout contiguous), tap flipped
+//   bd  bf16 [T][SliceP][CoutP]    wgmma B operand, dgrad    (K-major: Cout contiguous), tap flipped
 // one 16-bit element: bf16 or (half16) fp16 bits in the same slot
 __device__ __forceinline__ void st16(__nv_bfloat16* dst, float v, int half16) {
   if (half16) *reinterpret_cast<__half*>(dst) = __float2half_rn(v);
@@ -1427,7 +1427,7 @@ __global__ void __launch_bounds__(TPB) pack_split_weights_kernel(const float* __
 inline int grid_for(long long items) {
   long long b = (items + TPB - 1) / TPB;
   if (b < 1) b = 1;
-  if (b > 148 * 8) b = 148 * 8;
+  if (b > wsl_num_sms() * 8) b = wsl_num_sms() * 8;
   return (int)b;
 }
 
@@ -1435,7 +1435,7 @@ inline int bn_grid(long long P, int C, int per_sm = 3) {
   // every block should stream >= ~96 KB so that the fixed-order finalize (one pass over all partials) stays negligible
   long long b = (P * C * 2 + 96 * 1024 - 1) / (96 * 1024);
   if (b < 1) b = 1;
-  if (b > 148 * per_sm) b = 148 * per_sm;      // one full wave: 3 resident blocks / SM at 80 registers, 2 for the multi-source variants
+  if (b > wsl_num_sms() * per_sm) b = wsl_num_sms() * per_sm;      // one full wave: 3 resident blocks / SM at 80 registers, 2 for the multi-source variants
   return (int)b;
 }
 
@@ -1475,7 +1475,7 @@ WSL_API int wsl_wgrad_direct(const void* src0, int C0, const void* src1, int C1,
   const int Cin = C0 + C1;
   const int tx = (W + 15) / 16, ty = (H + 7) / 8;
   const int ob = (CoutP / 16) * ((Cin + 15) / 16);
-  int splits = (148 * 6 + ob - 1) / ob;
+  int splits = (wsl_num_sms() * 6 + ob - 1) / ob;
   const int ntiles = N * tx * ty;
   if (splits > ntiles) splits = ntiles;
   if (splits < 1) splits = 1;
@@ -1636,7 +1636,7 @@ WSL_API int wsl_bn_bwd_first(const void* y, int dtype, const float* ss, const fl
   unsigned* ticket = reinterpret_cast<unsigned*>(ws);
   const int grid = bn_grid(P, C, 3);
   int grid2 = (int)((P * 2 + TPB - 1) / TPB);
-  if (grid2 > 148) grid2 = 148;
+  if (grid2 > wsl_num_sms()) grid2 = wsl_num_sms();
   if (grid2 < 1) grid2 = 1;
   WSL_DISPATCH_T(dtype, {
     BnBwdArgs<T> a;
@@ -1764,7 +1764,7 @@ WSL_API int wsl_conv_first(const float* x, const float* w, const float* bias, vo
   WSL_REQUIRE(Cout == 16, "wsl_conv_first: compiled for 1 -> 16 channels (got Cout=%d)", Cout);
   WSL_REQUIRE((long long)N * H * W < (1LL << 30), "wsl_conv_first: too many pixels for 32-bit indexing");
   long long b = ((long long)N * H * ((W + 1) / 2) * 2 + TPB - 1) / TPB;
-  if (b > 148 * 4) b = 148 * 4;                  // one wave: four resident blocks per SM
+  if (b > wsl_num_sms() * 4) b = wsl_num_sms() * 4;                  // one wave: four resident blocks per SM
   if (b < 1) b = 1;
   WSL_DISPATCH_T(dtype, conv_first_kernel<T><<<(int)b, TPB, 0, stream>>>(x, w, bias, (T*)y, N, H, W, stat_partials));
   if (stat_rows_host) *stat_rows_host = (int)b;
@@ -1774,7 +1774,7 @@ WSL_API int wsl_conv_first(const float* x, const float* w, const float* bias, vo
 WSL_API int wsl_wgrad_first(const float* x, const void* dy, int dtype, float* dw, int N, int H, int W, int Cout, cudaStream_t stream) {
   WSL_REQUIRE(Cout == 16, "wsl_wgrad_first: compiled for 1 -> 16 channels (got Cout=%d)", Cout);
   long long b = ((long long)N * H * W + 256 * 16 - 1) / (256 * 16);
-  if (b > 148) b = 148;                      // x 2 channel halves x 2 resident blocks per SM = one wave
+  if (b > wsl_num_sms()) b = wsl_num_sms();                      // x 2 channel halves x 2 resident blocks per SM = one wave
   if (b < 1) b = 1;
   WSL_DISPATCH_T(dtype, wgrad_first_kernel<T><<<dim3((int)b, 2), 256, 0, stream>>>(x, (const T*)dy, dw, N, H, W));
   return wsl_check_launch("wgrad_first");

@@ -193,7 +193,7 @@ class BaseDataSets(torch.utils.data.Dataset):
     after `transform`; split='val': one sample per volume of the fold's test patients, ``{'image': [D,h,w], 'label': [D,h,w],
     'idx'}``.  Samples are produced on the HOST (numpy): the scripts iterate this object inside ``DataLoader(num_workers=8)``
     worker processes, which must not touch the GPU.  ``to_slice_store()`` hands the same slices to the resident GPU pipeline
-    (`SliceStore` / `GpuLoader`), which is what keeps up with the B200 step.
+    (`SliceStore` / `GpuLoader`), which is what keeps up with the training step.
 
     base_dir: the ACDC directory (``ACDC_training_slices/*.h5`` with datasets image / label / scribble and
     ``ACDC_training_volumes/*.h5``; needs h5py), or ``'synthetic'`` / ``'synthetic:<patients>'`` for the deterministic

@@ -5,7 +5,7 @@ The reference builds its network out of per-layer nn.Modules and lets autograd w
 shapes and init order, so state_dicts interchange); the arithmetic is a fixed launch sequence over
 preallocated channels-last bf16 buffers:
 
-  forward   conv (tcgen05 implicit GEMM, or CUDA-core direct for Cin=1 / tiny maps) -> BN statistics ->
+  forward   conv (wgmma implicit GEMM, or CUDA-core direct for Cin=1 / tiny maps) -> BN statistics ->
             BN-affine + LeakyReLU + dropout (+ fused 2x2 max-pool)      [x2 per ConvBlock]
             decoder: conv1x1 -> bilinear x2 -> two-source conv (concat never materialised)
   backward  BN backward (fused with LeakyReLU/dropout/max-pool routing and the skip/aux/pool gradient sum)
@@ -31,7 +31,7 @@ BF16 = torch.bfloat16
 LRELU_SLOPE = 0.01
 
 # execution modes: storage type of activations / activation gradients and the convolution kernels they run on
-#   bf16    (dtype code 0) tcgen05 kind::f16 on bf16 operands -- the throughput mode (BASELINE config 2 names bf16)
+#   bf16    (dtype code 0) wgmma on bf16 operands -- the throughput mode (BASELINE config 2 names bf16)
 #   fp16    (dtype code 2) the same kernels on fp16 operands (11-bit mantissa, identical MMA rate); gradients travel
 #           multiplied by a power-of-two loss scale so that they stay inside fp16's range
 #   fp16x3  (dtype code 1) fp32 storage; every convolution on the tensor cores with fp16 hi/lo split operands
@@ -329,7 +329,7 @@ class UNetExecutor:
         return (self.dt != 1 and self.use_tc and all(c % 16 == 0 for c in layer_cin_list) and W % 16 == 0 and H % 8 == 0)
 
     def _split_ok(self, layer_cin_list, H, W):
-        """fp16 hi/lo split convolutions (fp16x3 mode): the per-tap tcgen05 kernel's 16 x 8 pixel tiles"""
+        """fp16 hi/lo split convolutions (fp16x3 mode): the per-tap wgmma kernel's 16 x 8 pixel tiles"""
         return self.split_tc and self.use_tc and all(c % 16 == 0 for c in layer_cin_list) and W % 16 == 0 and H % 8 == 0
 
     def _staged(self, name, srcs, chans, P):
@@ -344,7 +344,7 @@ class UNetExecutor:
         return t[0], t[1][1:]
 
     def conv_fwd(self, L: ConvLayer, srcs, out, out_mode, N, H, W, cout_store, src_f32=False, bn_out=None, srcC_override=None):
-        """bn_out = (save, ss) buffers: when the convolution runs on the persistent tcgen05 kernel the complete
+        """bn_out = (save, ss) buffers: when the convolution runs on the persistent wgmma kernel the complete
         training-mode BatchNorm statistics of its output are produced by the kernel itself (partial rows in the epilogue,
         finalised by the last CTA).  Returns True when that happened."""
         pk = L.packs(self.dev)
@@ -378,7 +378,7 @@ class UNetExecutor:
             st, inv = self._staged("x", srcs, srcC, N * H * W)
             call("wsl_conv_tc_split", st, L.Cin, inv, pk["f3"], pk["bias"], out, out_mode, N, H, W, L.CoutP, cout_store, L.ks, L.dil)
         elif not src_f32 and L.dil != 1:
-            assert self._tc_ok(srcC, H, W), "dilated convolutions run on the per-tap tcgen05 kernel (W % 16 == 0, H % 8 == 0, 16-bit or fp16x3 mode)"
+            assert self._tc_ok(srcC, H, W), "dilated convolutions run on the per-tap wgmma kernel (W % 16 == 0, H % 8 == 0, 16-bit or fp16x3 mode)"
             call("wsl_conv_tc_dil", s0, c0, s1, c1, pk["bf"], pk["bias"], out, 0 if out_mode == 3 else out_mode, N, H, W, L.CoutP,
                  cout_store, L.ks, self.dt, L.dil)
         elif not src_f32 and self._tc2_ok(srcC, H, W):
@@ -414,7 +414,7 @@ class UNetExecutor:
             st, inv = self._staged("dy", [dy], [L.CoutP], N * H * W)
             call("wsl_conv_tc_split", st, L.CoutP, inv, pk["d3"][i], None, out, 2, N, H, W, sp, ci, L.ks, L.dil)
         elif L.dil != 1:
-            assert self._tc_ok([L.CoutP], H, W), "dilated data gradient: per-tap tcgen05 kernel only"
+            assert self._tc_ok([L.CoutP], H, W), "dilated data gradient: per-tap wgmma kernel only"
             call("wsl_conv_tc_dil", dy, L.CoutP, None, 0, pk["bd"][i], None, out, 0, N, H, W, sp, ci, L.ks, self.dt, L.dil)
         elif self._tc2_ok([L.CoutP], H, W):
             call("wsl_conv_tc2", dy, L.CoutP, None, 0, pk["bd"][i], None, out, 0, N, H, W, sp, ci, L.ks, self.dt, None, None)
@@ -443,7 +443,7 @@ class UNetExecutor:
             call("wsl_wgrad_tc_split", sx, L.Cin, ix, sg, L.CoutP, ig, self.gview(L.conv.weight), N, H, W, L.Cout, L.ks, L.dil)
             tc = True
         elif L.dil != 1 and not src_f32:
-            assert tc, "dilated weight gradient: per-tap tcgen05 kernel only"
+            assert tc, "dilated weight gradient: per-tap wgmma kernel only"
             pw = self._wgrad_partials() if self.deterministic_wgrad else None
             call("wsl_wgrad_tc_dil", s0, c0, s1, c1, dy, L.CoutP, self.gview(L.conv.weight), N, H, W, L.Cout, L.ks, self.dt, L.dil, pw,
                  pw.numel() if pw is not None else 0)

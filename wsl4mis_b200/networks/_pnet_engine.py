@@ -3,7 +3,7 @@
 Five blocks of two DILATED 3x3 convolutions (dilation = padding = 1, 2, 4, 8, 16) + BatchNorm + LeakyReLU at full resolution, the
 concatenation of the five block outputs, two 1x1 convolutions with LeakyReLU and no BatchNorm, and the output block
 Dropout2d(0.3) -> conv1x1 -> LeakyReLU -> Dropout2d(0.3) -> conv1x1.  Everything runs on the kernels of the U-Net executor: the
-dilated convolutions on the per-tap tcgen05 kernel (a tap is the TMA box at (y + d*dy, x + d*dx); zero fill = padding), the 1x1
+dilated convolutions on the per-tap wgmma kernel (a tap is the TMA box at (y + d*dy, x + d*dx); zero fill = padding), the 1x1
 convolutions on the persistent resident-weight kernel, BatchNorm / LeakyReLU / channel dropout on the same elementwise kernels
 (LeakyReLU without BatchNorm: `wsl_lrelu_fwd` / `wsl_lrelu_bwd`).  Modes: bf16, fp16 and
 fp16x3 (fp32-accurate split operands); there is no dilated CUDA-core kernel, so the plain `fp32` cross-check mode is not offered.
@@ -62,7 +62,7 @@ class PNetExecutor(UNetExecutor):
     def forward(self, x, training, need_grad, masks=None, chan_keep=None, defer_join=False):
         assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == self.in_chns == 1
         N, _, H, W = x.shape
-        assert H % 8 == 0 and W % 16 == 0, "PNet2D on the tcgen05 kernels needs H % 8 == 0 and W % 16 == 0"
+        assert H % 8 == 0 and W % 16 == 0, "PNet2D on the wgmma kernels needs H % 8 == 0 and W % 16 == 0"
         self.dev = x.device
         if not hasattr(self, "seed_dev") or self.seed_dev.device != self.dev:
             from ._engine import initial_rng_counter

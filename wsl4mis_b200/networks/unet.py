@@ -155,7 +155,7 @@ class _PlannedNet(nn.Module):
 
     def set_precision(self, precision):
         """Execution mode of the fused executor (networks/_engine.py:PRECISIONS):
-          'bf16'   default: activations / activation gradients stored in bf16, tcgen05 kind::f16 convolutions;
+          'bf16'   default: activations / activation gradients stored in bf16, wgmma convolutions;
           'fp16'   the same kernels on fp16 storage (11-bit mantissa, same speed; gradients carry a power-of-two loss scale);
           'fp16x3' fp32 storage, tensor-core convolutions on fp16 hi/lo split operands: fp32-accurate (the reference computes
                    in fp32, networks/unet.py:18-26), a few times slower than bf16;

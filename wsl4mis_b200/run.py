@@ -1,4 +1,4 @@
-"""Launcher for the reference's UNCHANGED training scripts on the B200 modules:
+"""Launcher for the reference's UNCHANGED training scripts on the H100 modules:
 
     cd /path/to/WSL4MIS/code
     python -m wsl4mis_b200.run train_weakly_supervised_pCE_GatedCRFLoss_2D.py --model unet --batch_size 64 ...
