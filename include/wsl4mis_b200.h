@@ -43,6 +43,16 @@ int wsl_workspace_floats(void);
 int wsl_softmax_pce_fwd(const float* logits, const uint8_t* label, float* probs, int N, int C, int H, int W,
                         int ignore_index, float* out2, float* ws, cudaStream_t stream);
 
+/* Scribble2Label step head (train_s2l.py:123-147): softmax once, u-labels where scribble == 4 and weight[..., c] > thr_conf (the
+ * last qualifying class wins, :133-145; map written to ulab), both masked NLL means.  ctrl = {thr_conf, w_u} in device memory
+ * (w_u = 0 before thr_iter, 0.5 after).  out5 = {pCE, #labelled, CE_u, #u-labelled, loss}, loss = pCE (w_u == 0) or
+ * pCE + w_u * CE_u (NaN when no pixel qualifies, as torch).  weight: [N,H,W,4] fp32.  wsl_s2l_head_bwd: dlogits of that loss
+ * times `scale` (an empty u-support adds nothing), fp32 NCHW and / or NHWC-16 bf16 / fp16 as wsl_head_bwd. */
+int wsl_s2l_fwd(const float* logits, const uint8_t* scribble, const float* weight, const float* ctrl, int N, int C, int H, int W,
+                float* probs, uint8_t* ulab, float* out5, float* ws, cudaStream_t stream);
+int wsl_s2l_head_bwd(const float* probs, const uint8_t* scribble, const uint8_t* ulab, const float* stats5, const float* ctrl,
+                     float scale, int N, int C, int H, int W, float* dlogits, void* dlogits_nhwc16, int dtype16, cudaStream_t stream);
+
 /* d(w_ce*pCE + <gprobs*gprobs_scale, softmax(logits)>)/dlogits, times *grad_out (NULL -> 1).
  * Replaces autograd through softmax / log_softmax+nll_loss.  label/gprobs may be NULL.  Either output may be NULL:
  * dlogits = fp32 NCHW (API layout), dlogits_nhwc16 = channels-last bf16 / fp16 (dtype16 0 / 2) padded to 16 channels (the
@@ -134,6 +144,16 @@ int wsl_nearest_resize_bwd(const float* gdst, long long planes, int h, int w, in
 int wsl_augment_sample_bytes(void);
 int wsl_augment_batch(const float* images, const uint8_t* labels, const void* table, int B, int OH, int OW, float* out_img,
                       uint8_t* out_lab, cudaStream_t stream);
+/* Scribble2Label sample transform (dataloaders/dataset_s2l.py:103-153, RandomGenerator_s2l): the same index map applied to the
+ * image, the scribble (rotation fill = lab_cval; the reference's scipy default is 0, SURVEY F15) and the [h,w,4] fp32 prediction
+ * memory, read from a ragged channels-last store (4 floats per pixel at element 4*off) and written as [B,OH,OW,4]. */
+int wsl_augment_batch_s2l(const float* images, const uint8_t* scribbles, const float* weights, const void* table, int B, int OH,
+                          int OW, float* out_img, uint8_t* out_scr, float* out_weight, cudaStream_t stream);
+/* Scribble2Label ensemble refresh (train_s2l.py:221-243) for B slices (table rows: off, h, w) whose [B,4,S,S] fp32 logits come
+ * from one batched forward: softmax at the zoom(order 0) source pixel of every native pixel (zoom's out-of-range fill reads 0),
+ * then weights = alpha * p + one_minus_alpha * weights in fp32 (ragged channels-last memory, updated in place). */
+int wsl_s2l_refresh(const float* logits, const void* table, int B, int S, long long max_hw, float alpha, float one_minus_alpha,
+                    float* weights, cudaStream_t stream);
 
 /* ---- network operators (networks/unet.py) ---------------------------------------------------------------- */
 
@@ -233,6 +253,17 @@ int wsl_bn_stats(const void* y, int dtype, long long P, int C, const float* gamm
  * all-reduces them over the data-parallel ranks and finalises with wsl_bn_finalize(raw_sums, 1, P_global, ...). */
 int wsl_bn_eval_prepare(const float* gamma, const float* beta, const float* running_mean, const float* running_var,
                         float eps, int C, float* ss, cudaStream_t stream);
+/* Per-sample BatchNorm training statistics (the batch-1 train-mode forwards of train_s2l.py:221-228 run as one batch): every
+ * image of [N][HW][C] gets its own {mean, invstd} -> save [N][2C] and {scale, shift} -> ss [N][2C]; running statistics take the
+ * N sequential momentum updates in image order (unbiased variance, n = HW) and num_batches_tracked += N.  Two deterministic
+ * launches (per-image partial rows in ws, fixed-order double sums). */
+int wsl_bn_stats_ps(const void* y, int dtype, int N, int HW, int C, const float* gamma, const float* beta, float* running_mean,
+                    float* running_var, long long* num_batches_tracked, float momentum, float eps, float* save, float* ss, float* ws,
+                    cudaStream_t stream);
+/* wsl_bn_act_fwd with ss = per-image {scale, shift} [N][2C] from wsl_bn_stats_ps. */
+int wsl_bn_act_fwd_ps(const void* y, int dtype, const float* ss, int N, int H, int W, int C, float slope, float drop_p,
+                      const uint8_t* mask, unsigned long long seed, const unsigned long long* seed_ptr, void* act,
+                      void* pooled, uint8_t* pool_idx, cudaStream_t stream);
 
 /* BN-affine + LeakyReLU(slope) + Dropout(p) (unet.py:20-22) and, when pooled != NULL, MaxPool2d(2) (unet.py:38)
  * of the result.  mask: optional uint8 keep mask (NHWC); NULL -> counter RNG on `seed` (+ *seed_ptr when non-NULL, so a

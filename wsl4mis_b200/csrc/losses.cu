@@ -881,6 +881,133 @@ __global__ void __launch_bounds__(TPB) nearest_resize_bwd_kernel(const float* __
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Scribble2Label step head (train_s2l.py:123-147).  ctrl = {thr_conf, w_u} in device memory (one captured graph serves both
+// sides of thr_iter).  Per pixel, softmax once, then
+//   scribble < 4                         -> pCE term (CrossEntropyLoss(ignore_index=4), :106,:124)
+//   scribble == 4, weight[c] > thr_conf  -> u-label c, the LAST qualifying class wins (:133-145)          else u-label 4
+// out = {pCE, #labelled, CE_u, #u-labelled, loss}; loss = pCE before thr_iter (w_u == 0) and pCE + w_u * CE_u after it,
+// which is NaN when no pixel qualifies, as torch's mean over an empty selection.  The u-label map is written for the backward.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(TPB) s2l_fwd_kernel(const float* __restrict__ logits, const uint8_t* __restrict__ scribble,
+                                                      const float4* __restrict__ weight, const float* __restrict__ ctrl,
+                                                      float* __restrict__ probs, uint8_t* __restrict__ ulab, int HW, long long nquads,
+                                                      float* partials, unsigned* ticket, float* out) {
+  float acc[4] = {0.f, 0.f, 0.f, 0.f};   // nll sum, labelled count, u-nll sum, u-labelled count
+  const int qpi = HW >> 2;
+  const float thr = ctrl[0];
+  for (long long q = blockIdx.x * (long long)TPB + threadIdx.x; q < nquads; q += (long long)gridDim.x * TPB) {
+    const long long n = q / qpi;
+    const int r = (int)(q - n * qpi);
+    const float* base = logits + n * C4 * (long long)HW + r * 4;
+    float x[C4][4];
+#pragma unroll
+    for (int c = 0; c < C4; ++c) {
+      float4 v = ld4(base + (long long)c * HW);
+      x[c][0] = v.x; x[c][1] = v.y; x[c][2] = v.z; x[c][3] = v.w;
+    }
+    const long long pix = n * (long long)HW + r * 4;
+    const uchar4 s4 = *reinterpret_cast<const uchar4*>(scribble + pix);
+    const int scr[4] = {s4.x, s4.y, s4.z, s4.w};
+    int ul[4];
+    float p[C4][4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float m = fmaxf(fmaxf(x[0][j], x[1][j]), fmaxf(x[2][j], x[3][j]));
+      float e[C4], s = 0.f;
+#pragma unroll
+      for (int c = 0; c < C4; ++c) { e[c] = expf(x[c][j] - m); s += e[c]; }
+      const float inv = 1.0f / s;
+#pragma unroll
+      for (int c = 0; c < C4; ++c) p[c][j] = e[c] * inv;
+      int u = 4;
+      if (scr[j] == 4) {
+        const float4 w = weight[pix + j];
+        if (w.x > thr) u = 0;
+        if (w.y > thr) u = 1;
+        if (w.z > thr) u = 2;
+        if (w.w > thr) u = 3;
+      }
+      ul[j] = u;
+      const int t = scr[j] < C4 ? scr[j] : u;          // the two supports are disjoint
+      if (t < C4) {
+        const float xl = t == 0 ? x[0][j] : t == 1 ? x[1][j] : t == 2 ? x[2][j] : x[3][j];
+        const float nll = logf(s) - (xl - m);
+        if (scr[j] < C4) { acc[0] += nll; acc[1] += 1.f; } else { acc[2] += nll; acc[3] += 1.f; }
+      }
+    }
+    float* pb = probs + n * C4 * (long long)HW + r * 4;
+#pragma unroll
+    for (int c = 0; c < C4; ++c) st4(pb + (long long)c * HW, make_float4(p[c][0], p[c][1], p[c][2], p[c][3]));
+    *reinterpret_cast<uchar4*>(ulab + pix) = make_uchar4((uint8_t)ul[0], (uint8_t)ul[1], (uint8_t)ul[2], (uint8_t)ul[3]);
+  }
+  __shared__ double res[4];
+  if (block_reduce_final<4, TPB>(acc, partials, ticket, res)) {
+    if (threadIdx.x == 0) {
+      const float ce = (float)(res[0] / res[1]), ce_u = (float)(res[2] / res[3]);   // 0 / 0 -> NaN, as torch
+      const float wu = ctrl[1];
+      out[0] = ce;
+      out[1] = (float)res[1];
+      out[2] = ce_u;
+      out[3] = (float)res[3];
+      out[4] = wu != 0.f ? ce + wu * ce_u : ce;
+    }
+  }
+}
+
+// dlogits of pCE + w_u * CE_u: (p - onehot(scribble)) * S / #labelled on scribbled pixels, (p - onehot(u)) * w_u * S / #u-labelled on
+// u-labelled ones, 0 elsewhere.  An empty u-support contributes nothing (torch's gradient of a NaN mean over no pixel is zero).
+// Output: fp32 NCHW and / or the executor's channels-last 16-channel bf16 / fp16 layout (as head_bwd_kernel).
+__global__ void __launch_bounds__(TPB) s2l_head_bwd_kernel(const float* __restrict__ probs, const uint8_t* __restrict__ scribble,
+                                                           const uint8_t* __restrict__ ulab, const float* __restrict__ stats,
+                                                           const float* __restrict__ ctrl, float scale, int HW, long long nquads,
+                                                           float* __restrict__ dlogits, __nv_bfloat16* __restrict__ dl_nhwc16, int dt16) {
+  const int qpi = HW >> 2;
+  const float cew = scale / stats[1];
+  const float wu = ctrl[1];
+  const float cuw = wu != 0.f ? wu * scale / stats[3] : 0.f;
+  for (long long q = blockIdx.x * (long long)TPB + threadIdx.x; q < nquads; q += (long long)gridDim.x * TPB) {
+    const long long n = q / qpi;
+    const int r = (int)(q - n * qpi);
+    const long long off = n * C4 * (long long)HW + r * 4;
+    const long long pix = n * (long long)HW + r * 4;
+    float p[C4][4];
+#pragma unroll
+    for (int c = 0; c < C4; ++c) {
+      float4 v = ld4(probs + off + (long long)c * HW);
+      p[c][0] = v.x; p[c][1] = v.y; p[c][2] = v.z; p[c][3] = v.w;
+    }
+    const uchar4 s4 = *reinterpret_cast<const uchar4*>(scribble + pix);
+    const uchar4 u4 = *reinterpret_cast<const uchar4*>(ulab + pix);
+    const int scr[4] = {s4.x, s4.y, s4.z, s4.w}, ul[4] = {u4.x, u4.y, u4.z, u4.w};
+    float d[C4][4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const bool lab = scr[j] < C4;
+      const int t = lab ? scr[j] : ul[j];
+      const float w = lab ? cew : (t < C4 ? cuw : 0.f);
+#pragma unroll
+      for (int c = 0; c < C4; ++c) d[c][j] = (w != 0.f) ? w * (p[c][j] - (t == c ? 1.f : 0.f)) : 0.f;
+    }
+    if (dlogits != nullptr) {
+#pragma unroll
+      for (int c = 0; c < C4; ++c) st4(dlogits + off + (long long)c * HW, make_float4(d[c][0], d[c][1], d[c][2], d[c][3]));
+    }
+    if (dl_nhwc16 != nullptr) {
+      uint4* o = reinterpret_cast<uint4*>(dl_nhwc16 + pix * 16);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        uint4 v;
+        v.x = dt16 == 2 ? pack_f16(d[0][j], d[1][j]) : pack_bf16(d[0][j], d[1][j]);
+        v.y = dt16 == 2 ? pack_f16(d[2][j], d[3][j]) : pack_bf16(d[2][j], d[3][j]);
+        v.z = 0u; v.w = 0u;
+        o[2 * j] = v;
+        o[2 * j + 1] = make_uint4(0u, 0u, 0u, 0u);
+      }
+    }
+  }
+}
+
 inline int grid_for(long long work_items, int per_block) {
   long long b = (work_items + per_block - 1) / per_block;
   if (b < 1) b = 1;
@@ -1089,4 +1216,25 @@ WSL_API int wsl_nearest_resize_fwd(const float* src, long long planes, int h, in
 WSL_API int wsl_nearest_resize_bwd(const float* gdst, long long planes, int h, int w, int H, int W, float* gsrc, cudaStream_t stream) {
   nearest_resize_bwd_kernel<<<grid_for(planes * h * w, TPB), TPB, 0, stream>>>(gdst, planes, h, w, H, W, gsrc);
   return wsl_check_launch("nearest_resize_bwd");
+}
+
+WSL_API int wsl_s2l_fwd(const float* logits, const uint8_t* scribble, const float* weight, const float* ctrl, int N, int C, int H, int W,
+                        float* probs, uint8_t* ulab, float* out5, float* ws, cudaStream_t stream) {
+  WSL_REQUIRE(C == C4, "wsl_s2l_fwd: C must be 4 (got %d)", C);
+  WSL_REQUIRE(((long long)H * W) % 4 == 0, "wsl_s2l_fwd: H*W must be a multiple of 4");
+  WSL_REQUIRE(((uintptr_t)weight & 15) == 0, "wsl_s2l_fwd: weight must be 16-byte aligned");
+  const long long nq = (long long)N * H * W / 4;
+  s2l_fwd_kernel<<<grid_for(nq, TPB), TPB, 0, stream>>>(logits, scribble, reinterpret_cast<const float4*>(weight), ctrl, probs, ulab, H * W,
+                                                        nq, ws + 64, reinterpret_cast<unsigned*>(ws), out5);
+  return wsl_check_launch("s2l_fwd");
+}
+
+WSL_API int wsl_s2l_head_bwd(const float* probs, const uint8_t* scribble, const uint8_t* ulab, const float* stats5, const float* ctrl,
+                             float scale, int N, int C, int H, int W, float* dlogits, void* dlogits_nhwc16, int dtype16, cudaStream_t stream) {
+  WSL_REQUIRE(C == C4, "wsl_s2l_head_bwd: C must be 4 (got %d)", C);
+  WSL_REQUIRE(((long long)H * W) % 4 == 0, "wsl_s2l_head_bwd: H*W must be a multiple of 4");
+  const long long nq = (long long)N * H * W / 4;
+  s2l_head_bwd_kernel<<<grid_for(nq, TPB), TPB, 0, stream>>>(probs, scribble, ulab, stats5, ctrl, scale, H * W, nq, dlogits,
+                                                             (__nv_bfloat16*)dlogits_nhwc16, dtype16);
+  return wsl_check_launch("s2l_head_bwd");
 }

@@ -538,6 +538,68 @@ __global__ void __launch_bounds__(TPB) bn_finalize_kernel(const float* __restric
   if (blockIdx.x == 0 && threadIdx.x == 0 && nbt) *nbt += 1;
 }
 
+// ---- per-sample BatchNorm (training statistics of every image on its own) ---------------------------------------------
+// For the Scribble2Label ensemble refresh (train_s2l.py:221-228): B batch-1 training forwards in one batched pass.  Pass 1: grid
+// (blocks per image, N), the layout of bn_stats_kernel restricted to one image's HW pixels, partials [N][nblk][2][C].  Pass 2:
+// one thread per channel walks the images in order (fixed-order double sums as bn_finalize_kernel), writes {mean, invstd} and
+// {scale, shift} per image, and applies the N running-statistics updates in slice order (unbiased variance with n = HW).
+template <typename T>
+__global__ void __launch_bounds__(TPB) bn_stats_ps_kernel(const T* __restrict__ y, int HW, int C, float* __restrict__ partials) {
+  extern __shared__ float s_red[];  // [TPB][16]
+  const int cg = C >> 3, rows = TPB / cg;
+  const int g = threadIdx.x % cg, r = threadIdx.x / cg;
+  const T* yn = y + (size_t)blockIdx.y * HW * C;
+  float sum[8], sq[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) sum[j] = sq[j] = 0.f;
+  for (int p = blockIdx.x * rows + r; p < HW; p += gridDim.x * rows) {
+    float v[8];
+    ld8(yn + (size_t)p * C + g * 8, v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { sum[j] += v[j]; sq[j] = fmaf(v[j], v[j], sq[j]); }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) { s_red[threadIdx.x * 16 + j] = sum[j]; s_red[threadIdx.x * 16 + 8 + j] = sq[j]; }
+  __syncthreads();
+  float* part = partials + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 2 * C;
+  for (int c = threadIdx.x; c < C; c += TPB) {
+    const int gg = c >> 3, j = c & 7;
+    float a = 0.f, b = 0.f;
+    for (int rr = 0; rr < rows; ++rr) { a += s_red[(rr * cg + gg) * 16 + j]; b += s_red[(rr * cg + gg) * 16 + 8 + j]; }
+    part[c] = a;
+    part[C + c] = b;
+  }
+}
+
+__global__ void __launch_bounds__(TPB) bn_finalize_ps_kernel(const float* __restrict__ partials, int nblk, int N, int HW, int C,
+                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                             float* running_mean, float* running_var, long long* nbt, float momentum,
+                                                             float eps, float* __restrict__ save, float* __restrict__ ss) {
+  const int c = blockIdx.x * TPB + threadIdx.x;
+  if (c < C) {
+    float rm = running_mean ? running_mean[c] : 0.f, rv = running_var ? running_var[c] : 0.f;
+    for (int n = 0; n < N; ++n) {
+      const float* part = partials + (size_t)n * nblk * 2 * C;
+      double a = 0.0, b = 0.0;
+      for (int bl = 0; bl < nblk; ++bl) { a += (double)part[(size_t)bl * 2 * C + c]; b += (double)part[(size_t)bl * 2 * C + C + c]; }
+      const double mean = a / (double)HW;
+      double var = b / (double)HW - mean * mean;
+      if (var < 0.0) var = 0.0;
+      const float invstd = (float)(1.0 / sqrt(var + (double)eps));
+      const float sc = gamma[c] * invstd;
+      save[(size_t)n * 2 * C + c] = (float)mean;
+      save[(size_t)n * 2 * C + C + c] = invstd;
+      ss[(size_t)n * 2 * C + c] = sc;
+      ss[(size_t)n * 2 * C + C + c] = beta[c] - (float)mean * sc;
+      const double unb = (HW > 1) ? var * (double)HW / (double)(HW - 1) : var;
+      rm = (1.f - momentum) * rm + momentum * (float)mean;
+      rv = (1.f - momentum) * rv + momentum * (float)unb;
+    }
+    if (running_mean) { running_mean[c] = rm; running_var[c] = rv; }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0 && nbt) *nbt += N;
+}
+
 // eval mode: scale/shift from running statistics
 __global__ void bn_eval_prepare_kernel(const float* gamma, const float* beta, const float* rm, const float* rv,
                                        float eps, int C, float* ss) {
@@ -602,7 +664,8 @@ struct BnFin {
 };
 
 // A = dropout(leaky_relu(y*scale + shift)); optional fused 2x2 max-pool of A (DownBlock, unet.py:38).
-template <typename T>
+// PER_SAMPLE: ss holds {scale, shift} per image, [N][2][C] (per-sample BatchNorm, bn_stats_ps_kernel); reloaded when the pixel's image changes.
+template <typename T, bool PER_SAMPLE = false>
 __global__ void __launch_bounds__(TPB) bn_act_fwd_kernel(
     const T* __restrict__ y, const float* __restrict__ ss, int N, int H, int W, int C, float slope,
     float drop_p, const uint8_t* __restrict__ mask, unsigned long long seed, const unsigned long long* seed_ptr,
@@ -661,7 +724,16 @@ __global__ void __launch_bounds__(TPB) bn_act_fwd_kernel(
     for (int j = 0; j < 8; ++j) { sc[j] = ss[c0 + j]; sh[j] = ss[C + c0 + j]; }
   }
   // loads are issued for all pixels of an iteration before the first use (the dropout branch would otherwise serialise them)
+  int cur_n = 0;
   auto act8 = [&](int p, const float (&v)[8], float (&o)[8]) {
+    if constexpr (PER_SAMPLE) {
+      const int n = p / (H * W);
+      if (n != cur_n) {
+        cur_n = n;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { sc[j] = ss[(size_t)n * 2 * C + c0 + j]; sh[j] = ss[(size_t)n * 2 * C + C + c0 + j]; }
+      }
+    }
     const uint32_t kb = keep_bits8(dc, (long long)p * C + c0, (uint32_t)p * cg + g);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -1793,4 +1865,35 @@ WSL_API int wsl_bn_finalize(const float* partials, int nrows, long long P, int C
   bn_finalize_kernel<<<(C + 15) / 16, TPB, 0, stream>>>(partials, nrows, P, C, gamma, beta, running_mean, running_var, num_batches_tracked,
                                             momentum, eps, save, ss);
   return wsl_check_launch("bn_finalize");
+}
+
+WSL_API int wsl_bn_stats_ps(const void* y, int dtype, int N, int HW, int C, const float* gamma, const float* beta, float* running_mean,
+                            float* running_var, long long* num_batches_tracked, float momentum, float eps, float* save, float* ss, float* ws,
+                            cudaStream_t stream) {
+  WSL_REQUIRE(C % 8 == 0 && C <= 256 && TPB % (C / 8) == 0, "wsl_bn_stats_ps: unsupported channel count %d", C);
+  WSL_REQUIRE(N > 0 && N <= 65535 && HW > 0, "wsl_bn_stats_ps: bad shape (N=%d, HW=%d)", N, HW);
+  long long nblk = ((long long)HW * C + 65535) / 65536;      // ~64 K elements per block
+  if (nblk > 32) nblk = 32;
+  if (nblk < 1) nblk = 1;
+  WSL_REQUIRE((long long)N * nblk * 2 * C <= WSL_WS_FLOATS, "wsl_bn_stats_ps: workspace too small for N=%d, C=%d", N, C);
+  WSL_DISPATCH_T(dtype, bn_stats_ps_kernel<T><<<dim3((unsigned)nblk, (unsigned)N), TPB, TPB * 16 * sizeof(float), stream>>>((const T*)y, HW, C, ws));
+  if (const int rc = wsl_check_launch("bn_stats_ps")) return rc;
+  bn_finalize_ps_kernel<<<(C + TPB - 1) / TPB, TPB, 0, stream>>>(ws, (int)nblk, N, HW, C, gamma, beta, running_mean, running_var,
+                                                                 num_batches_tracked, momentum, eps, save, ss);
+  return wsl_check_launch("bn_finalize_ps");
+}
+
+WSL_API int wsl_bn_act_fwd_ps(const void* y, int dtype, const float* ss, int N, int H, int W, int C, float slope, float drop_p,
+                              const uint8_t* mask, unsigned long long seed, const unsigned long long* seed_ptr, void* act,
+                              void* pooled, uint8_t* pool_idx, cudaStream_t stream) {
+  WSL_REQUIRE(C % 8 == 0, "wsl_bn_act_fwd_ps: C %% 8 != 0");
+  WSL_REQUIRE(pooled == nullptr || (H % 2 == 0 && W % 2 == 0), "wsl_bn_act_fwd_ps: pooling needs even H, W");
+  WSL_REQUIRE(TPB % (C / 8) == 0 && (long long)N * H * W < (1LL << 31), "wsl_bn_act_fwd_ps: unsupported C=%d or too many pixels", C);
+  BnFin fin;
+  fin.partials = nullptr; fin.nrows = 0; fin.P = 0; fin.gamma = fin.beta = nullptr; fin.running_mean = fin.running_var = nullptr;
+  fin.nbt = nullptr; fin.momentum = 0.f; fin.eps = 0.f; fin.save = fin.ss_out = nullptr;
+  const long long items = (long long)N * H * W * (C / 8) / (pooled ? 4 : 1);
+  WSL_DISPATCH_T(dtype, (bn_act_fwd_kernel<T, true><<<grid_for((items + 1) / 2), TPB, 0, stream>>>(
+                            (const T*)y, ss, N, H, W, C, slope, drop_p, mask, seed, seed_ptr, (T*)act, (T*)pooled, pool_idx, fin)));
+  return wsl_check_launch("bn_act_fwd_ps");
 }

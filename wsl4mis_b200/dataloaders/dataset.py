@@ -8,6 +8,7 @@ maps, and the random parameters are drawn on the host from the same ``random`` /
 order as the reference's transform, so a batch is bit-identical to what the reference pipeline produces for the same
 draws (tests/test_gpu_data.py).
 """
+import collections
 import os
 import random
 
@@ -80,19 +81,55 @@ def apply_host(image, label, params, output_size):
     return image.astype(np.float32), label.astype(np.uint8)
 
 
-class SliceStore:
-    """All training slices resident on the GPU: flat fp32 images, flat uint8 labels, per-slice offset / shape."""
+class RandomGenerator_s2l:
+    """``RandomGenerator_s2l(output_size)`` of dataset_s2l.py:126-153, on the HOST for DataLoader workers: the draws of
+    `RandomGenerator` (:132-137); image, mask, scribble and the [h,w,4] weight through the same rot90 / flip / rotate(order 0,
+    cval 0 for every array -- the scribble's rotated-in corners become background, SURVEY F15) and zoom(order 0; factor 1 on the
+    class axis).  `SliceStore.augment_s2l` produces the same samples on the GPU for the same draws."""
 
-    def __init__(self, images, labels, offs, shapes, has4, names):
+    def __init__(self, output_size):
+        self.output_size = tuple(int(v) for v in output_size)
+
+    def __call__(self, sample):
+        params = RandomGenerator.draw(False)
+        image = np.asarray(sample["image"], dtype=np.float32)
+        img, mask = apply_host(image, np.asarray(sample["mask"]).astype(np.uint8), params, self.output_size)
+        _, scr = apply_host(image, np.asarray(sample["scribble"]).astype(np.uint8), params, self.output_size)
+        weight = np.asarray(sample["weight"], dtype=np.float32)
+        wgt = np.stack([apply_host(weight[..., c], mask, params, self.output_size)[0] for c in range(weight.shape[2])], -1)
+        return {"image": torch.from_numpy(img).unsqueeze(0), "mask": torch.from_numpy(mask), "scribble": torch.from_numpy(scr),
+                "weight": torch.from_numpy(np.ascontiguousarray(wgt, dtype=np.float32))}
+
+
+class SliceStore:
+    """All training slices resident on the GPU: flat fp32 images, flat uint8 labels, per-slice offset / shape.
+
+    With ``scribbles`` (Scribble2Label, dataset_s2l.py:34-46) the store also holds the scribble maps and the per-slice 4-class
+    prediction memory, zero-initialised like :46, as ragged channels-last fp32 ([pixels, 4]) in two copies: ``weight_live``,
+    which the ensemble refresh updates, and ``weight_epoch``, the snapshot training batches read (SURVEY F16)."""
+
+    def __init__(self, images, labels, offs, shapes, has4, names, scribbles=None):
         self.images, self.labels = images, labels
         self.offs, self.shapes, self.has4, self.names = offs, shapes, has4, names
         assert LIB.load().wsl_augment_sample_bytes() == _SAMPLE.itemsize, "AugSample layout mismatch"
+        self.scribbles = scribbles
+        self.weight_live = self.weight_epoch = None
+        if scribbles is not None:
+            assert scribbles.numel() == images.numel()
+            self.weight_live = torch.zeros(images.numel(), 4, dtype=torch.float32, device=images.device)
+            self.weight_epoch = torch.zeros_like(self.weight_live)
+
+    def weight(self, i, which="live"):
+        """the [h, w, 4] prediction memory of slice i (a view)"""
+        h, w = int(self.shapes[i, 0]), int(self.shapes[i, 1])
+        mem = self.weight_live if which == "live" else self.weight_epoch
+        return mem[self.offs[i]: self.offs[i] + h * w].view(h, w, 4)
 
     def __len__(self):
         return len(self.offs)
 
     @classmethod
-    def from_arrays(cls, images, labels, names=None, device=None):
+    def from_arrays(cls, images, labels, names=None, device=None, scribbles=None):
         device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         assert len(images) == len(labels) and len(images) > 0
         shapes = np.array([im.shape for im in images], dtype=np.int32)
@@ -104,7 +141,11 @@ class SliceStore:
         flat_l = np.concatenate([np.asarray(lb).astype(np.uint8).ravel() for lb in labels])
         has4 = np.array([bool((np.asarray(lb) == 4).any()) for lb in labels])
         names = list(names) if names is not None else [str(i) for i in range(len(images))]
-        return cls(torch.from_numpy(flat_i).to(device), torch.from_numpy(flat_l).to(device), offs, shapes, has4, names)
+        flat_s = None
+        if scribbles is not None:
+            assert len(scribbles) == len(images) and all(np.shape(sc) == im.shape for sc, im in zip(scribbles, images))
+            flat_s = torch.from_numpy(np.concatenate([np.asarray(sc).astype(np.uint8).ravel() for sc in scribbles])).to(device)
+        return cls(torch.from_numpy(flat_i).to(device), torch.from_numpy(flat_l).to(device), offs, shapes, has4, names, flat_s)
 
     @classmethod
     def from_h5_dir(cls, base_dir, cases, sup_type="scribble", device=None):
@@ -120,8 +161,8 @@ class SliceStore:
                 lbs.append(f[sup_type][:])
         return cls.from_arrays(ims, lbs, [c.split("_")[0] for c in cases], device)
 
-    def augment(self, indices, params, output_size):
-        """indices: slice ids; params: (mode, k, axis, angle, lab_cval) per sample -> (image [B,1,H,W] fp32, label [B,H,W] u8)."""
+    def table(self, indices, params):
+        """AugSample rows (device, bytes) of the samples: slice ids and (mode, k, axis, angle, lab_cval) per sample."""
         B = len(indices)
         tab = np.zeros(B, dtype=_SAMPLE)
         for b, (i, (mode, k, axis, angle, cval)) in enumerate(zip(indices, params)):
@@ -133,13 +174,31 @@ class SliceStore:
                 rot, off = _rotation(angle, (h, w))
                 row["m00"], row["m01"], row["m10"], row["m11"] = rot[0, 0], rot[0, 1], rot[1, 0], rot[1, 1]
                 row["o0"], row["o1"] = off[0], off[1]
-        dev = self.images.device
-        tab_d = torch.from_numpy(tab.view(np.uint8)).to(dev, non_blocking=True)
+        return torch.from_numpy(tab.view(np.uint8)).to(self.images.device, non_blocking=True)
+
+    def augment(self, indices, params, output_size):
+        """indices: slice ids; params: (mode, k, axis, angle, lab_cval) per sample -> (image [B,1,H,W] fp32, label [B,H,W] u8)."""
+        B, dev = len(indices), self.images.device
+        tab_d = self.table(indices, params)
         OH, OW = output_size
         img = torch.empty(B, 1, OH, OW, dtype=torch.float32, device=dev)
         lab = torch.empty(B, OH, OW, dtype=torch.uint8, device=dev)
         call("wsl_augment_batch", self.images, self.labels, tab_d, B, OH, OW, img, lab)
         return img, lab
+
+    def augment_s2l(self, indices, params, output_size, which="epoch"):
+        """RandomGenerator_s2l (dataset_s2l.py:126-153) for a batch: -> (image [B,1,H,W] fp32, scribble [B,H,W] u8,
+        weight [B,H,W,4] fp32) gathered in one launch from the scribble store and the `which` ('epoch' | 'live') memory."""
+        assert self.scribbles is not None, "this store has no scribbles / prediction memory (from_arrays(..., scribbles=))"
+        B, dev = len(indices), self.images.device
+        tab_d = self.table(indices, params)
+        OH, OW = output_size
+        img = torch.empty(B, 1, OH, OW, dtype=torch.float32, device=dev)
+        scr = torch.empty(B, OH, OW, dtype=torch.uint8, device=dev)
+        wgt = torch.empty(B, OH, OW, 4, dtype=torch.float32, device=dev)
+        mem = self.weight_epoch if which == "epoch" else self.weight_live
+        call("wsl_augment_batch_s2l", self.images, self.scribbles, mem, tab_d, B, OH, OW, img, scr, wgt)
+        return img, scr, wgt
 
 
 def fold_ids(fold):
@@ -257,6 +316,76 @@ class BaseDataSets(torch.utils.data.Dataset):
         return SliceStore.from_arrays([p[0] for p in pairs], [p[1] for p in pairs], [c.split("_")[0] for c in self.sample_list], device)
 
 
+class TwoStreamBatchSampler(torch.utils.data.Sampler):
+    """Batch sampler of the reference's semi-supervised scripts (imported by train_s2l.py:20): every batch is
+    ``batch_size - secondary_batch_size`` indices of `primary_indices`, walked once per epoch in a fresh numpy permutation, followed
+    by `secondary_batch_size` indices of `secondary_indices`, cycled through as many fresh permutations as the epoch needs.  An
+    epoch has len(primary_indices) // primary batch size batches; a trailing partial primary batch is dropped."""
+
+    def __init__(self, primary_indices, secondary_indices, batch_size, secondary_batch_size):
+        self.primary_indices, self.secondary_indices = primary_indices, secondary_indices
+        self.secondary_batch_size = int(secondary_batch_size)
+        self.primary_batch_size = int(batch_size) - self.secondary_batch_size
+        if not 0 < self.primary_batch_size <= len(primary_indices):
+            raise ValueError(f"primary batch size {self.primary_batch_size} must be in [1, {len(primary_indices)}]")
+        if not 0 < self.secondary_batch_size <= len(secondary_indices):
+            raise ValueError(f"secondary batch size {self.secondary_batch_size} must be in [1, {len(secondary_indices)}]")
+
+    def __len__(self):
+        return len(self.primary_indices) // self.primary_batch_size
+
+    def _secondary(self):
+        while True:
+            yield from np.random.permutation(self.secondary_indices)
+
+    def __iter__(self):
+        primary = np.random.permutation(self.primary_indices)       # drawn when the epoch's iterator is created
+        secondary = self._secondary()
+        nb, sb = self.primary_batch_size, self.secondary_batch_size
+
+        def batches():
+            for b in range(len(self)):
+                yield tuple(primary[b * nb:(b + 1) * nb]) + tuple(next(secondary) for _ in range(sb))
+        return batches()
+
+
+class BaseDataSets_s2l(torch.utils.data.Dataset):
+    """``BaseDataSets_s2l(base_dir, transform, fold, num)`` of dataset_s2l.py:19-100: the fold's training slices held in memory as
+    ``images[idx] = {'id', 'image', 'mask', 'scribble', 'weight'}`` with a zero-initialised [h, w, 4] fp32 prediction memory
+    (:46) that train_s2l.py's ensemble refresh rewrites in place (:243).  base_dir as `BaseDataSets` (ACDC directory with h5py,
+    or 'synthetic[:<patients>]').  ``to_slice_store()`` hands the slices to the resident GPU pipeline (`S2LLoader`)."""
+
+    def __init__(self, base_dir=None, transform=None, fold="fold1", num=None):
+        src = BaseDataSets(base_dir, "train", None, fold, "label")     # `num` is accepted and ignored, as in the reference
+        self._base_dir, self.transform = base_dir, transform
+        self.sample_list = list(src.sample_list)
+        self.images = collections.defaultdict(dict)
+        for idx, case in enumerate(self.sample_list):
+            src.sup_type = "label"
+            img, mask = src._read(case)
+            src.sup_type = "scribble"
+            _, scr = src._read(case)
+            rec = self.images[idx]
+            rec["id"], rec["image"], rec["mask"], rec["scribble"] = case, np.asarray(img), np.asarray(mask), np.asarray(scr)
+            rec["weight"] = np.zeros(tuple(np.shape(mask)) + (4,), dtype=np.float32)
+
+    def __len__(self):
+        return len(self.sample_list)
+
+    def __getitem__(self, idx):
+        rec = self.images[idx]
+        sample = {"image": rec["image"], "mask": rec["mask"], "scribble": rec["scribble"], "weight": rec["weight"]}
+        sample = self.transform(sample)
+        sample["id"] = rec["id"]
+        return sample
+
+    def to_slice_store(self, device=None):
+        """the slices (mask as label, scribble, zero memory) as a resident GPU `SliceStore` for `S2LLoader` / `S2LStep.refresh`"""
+        recs = [self.images[i] for i in range(len(self))]
+        return SliceStore.from_arrays([r["image"] for r in recs], [r["mask"] for r in recs], [r["id"].split("_")[0] for r in recs],
+                                      device, scribbles=[r["scribble"] for r in recs])
+
+
 class GpuLoader:
     """Replaces ``DataLoader(db_train, batch_size, shuffle=True)`` + ``RandomGenerator`` for the training split: yields
     ``{'image': [B,1,H,W] fp32 cuda, 'label': [B,H,W] uint8 cuda, 'idx': [...]}`` (script keys, dataset_semi.py:120-124)."""
@@ -282,7 +411,8 @@ class GpuLoader:
         n = (len(self.store) + self.world_size - 1) // self.world_size
         return n // self.batch_size if self.drop_last else (n + self.batch_size - 1) // self.batch_size
 
-    def __iter__(self):
+    def _batches(self):
+        """slice ids of every batch of one epoch"""
         n = len(self.store)
         if self.shuffle:     # torch.utils.data.RandomSampler: fresh generator seeded from the default stream, then randperm
             seed = int(torch.empty((), dtype=torch.int64).random_().item())
@@ -297,6 +427,35 @@ class GpuLoader:
             idx = order[s:s + self.batch_size]
             if len(idx) < self.batch_size and self.drop_last:
                 break
+            yield idx
+
+    def __iter__(self):
+        for idx in self._batches():
             params = [self.transform.draw(bool(self.store.has4[i])) for i in idx]
             img, lab = self.store.augment(idx, params, self.transform.output_size)
             yield {"image": img, "label": lab, "idx": [self.store.names[i] for i in idx]}
+
+
+class S2LLoader(GpuLoader):
+    """Replaces ``DataLoader(BaseDataSets_s2l, batch_size, shuffle=True, num_workers=8)`` + ``RandomGenerator_s2l``
+    (train_s2l.py:86-99): yields ``{'image': [B,1,H,W] fp32, 'scribble': [B,H,W] u8, 'weight': [B,H,W,4] fp32, 'idx': [...]}``.
+
+    visibility='epoch' (default, SURVEY F16): the script's workers are forked when an epoch's iterator is created, so its
+    batches see the prediction memory as it was at that moment; the snapshot is taken when iteration starts and a refresh in
+    mid-epoch reaches the batches of the next epoch.  visibility='live': batches read the memory the refresh updates."""
+
+    def __init__(self, store, batch_size, output_size=(256, 256), shuffle=True, drop_last=False, visibility="epoch"):
+        assert store.scribbles is not None, "S2LLoader needs a SliceStore built with scribbles="
+        if visibility not in ("epoch", "live"):
+            raise ValueError(f"visibility must be 'epoch' or 'live' (got {visibility!r})")
+        super().__init__(store, batch_size, output_size, shuffle, drop_last)
+        self.visibility = visibility
+
+    def __iter__(self):
+        if self.visibility == "epoch":
+            self.store.weight_epoch.copy_(self.store.weight_live)
+        for idx in self._batches():
+            # the draws of RandomGenerator_s2l are RandomGenerator's; the scribble is rotated with cval 0 (SURVEY F15)
+            params = [self.transform.draw(False) for _ in idx]
+            img, scr, wgt = self.store.augment_s2l(idx, params, self.transform.output_size, self.visibility)
+            yield {"image": img, "scribble": scr, "weight": wgt, "idx": [self.store.names[i] for i in idx]}

@@ -8,7 +8,7 @@
   dmpls          train_weakly_supervised_segmentation_pCE_ours_proposed.py:108-132
   pce_entropy    train_weakly_supervised_pCE_Entropy_Mini_2D.py:97-109
   pce_variance   train_weakly_supervised_pCE_Inter&Intra_Class_2D.py:112-125 (weight = consistency * sigmoid_rampup(it//150, 200))
-as ONE launch sequence: executor forward -> fused loss head (softmax+pCE, regulariser, combined backward into
+(``S2LStep`` below adds Scribble2Label, train_s2l.py:119-157, and its ensemble refresh :214-243) as ONE launch sequence: executor forward -> fused loss head (softmax+pCE, regulariser, combined backward into
 dlogits) -> executor backward into a flat fp32 gradient bucket -> (NCCL all-reduce of that bucket when
 world_size > 1) -> fused SGD(momentum 0.9, wd 1e-4) over the flat parameter buffer with the poly LR read from
 device memory.  The whole sequence is CUDA-graph captured after the first call (graph=True).
@@ -667,3 +667,86 @@ class USTMStep(UAMTStep):
         self.parts = {"ce": st[0], "consistency": cst[2], "mask": mask}
         g = ex.backward(slot, [d] + [None] * (len(ex.dec) - 1))
         return loss, g
+
+
+class S2LStep(TrainStep):
+    """Per-step body of train_s2l.py:119-157 (Scribble2Label) on the fused kernels, plus its ensemble refresh (:214-243).
+
+    Step: pCE on the scribbles (ignore_index 4); from iteration `thr_iter` on (pre-increment counter, :125) plus 0.5 * CE on the
+    u-labels derived from the augmented prediction memory (`weight`, [B,H,W,4]) where scribble == 4 and weight > thr_conf.  Both
+    terms, their u-label map and the combined logit gradient come from two kernels; thr_conf and the before/after-thr_iter switch
+    live in device memory (`ctrl`), so graph=True captures one graph that serves the whole run.  SGD / poly LR as TrainStep.
+
+    Only single-output models run this script (softmax(model(img)), :228); multi-GPU Scribble2Label is not supported."""
+
+    def __init__(self, model, thr_iter=6000, thr_conf=0.8, base_lr=0.01, max_iterations=60000, momentum=0.9, weight_decay=1e-4,
+                 graph=True, world_size=1, **kw):
+        if int(world_size) != 1:
+            raise NotImplementedError("Scribble2Label runs on one GPU (world_size must be 1)")
+        ex = model.executor
+        if len(ex.dec) != 1 or any(ex.ds_heads) or not hasattr(ex, "enc_blocks"):
+            raise ValueError("Scribble2Label needs a single-output U-Net (train_s2l.py:228 takes softmax(model(img)))")
+        super().__init__(model, "pce", base_lr=base_lr, max_iterations=max_iterations, momentum=momentum, weight_decay=weight_decay,
+                         graph=graph, **kw)
+        self.thr_iter, self.thr_conf = int(thr_iter), float(thr_conf)
+        self.ctrl = torch.tensor([self.thr_conf, 0.0], dtype=torch.float32, device=self.dev)    # {thr_conf, w_u}
+        self._w_u = 0.0
+        self._weight = None
+        self._wstatic = None
+
+    def _head(self, logits_list, image, label, slot):
+        ex = self.ex
+        N, C, H, W = logits_list[0].shape
+        S = ex.grad_scale_for(N, H, W) if ex.dt != 1 else 1.0
+        probs = ex.buf(slot, "head.probs0", (N, C, H, W), torch.float32)
+        ulab = ex.buf(slot, "head.ulab", (N, H, W), torch.uint8)
+        st = ex.buf(slot, "head.s2l", (5,), torch.float32)
+        call("wsl_s2l_fwd", logits_list[0], label, self._weight, self.ctrl, N, C, H, W, probs, ulab, st, workspace("s2l", self.dev))
+        d, d16, dl0 = self._dlogits(ex, slot, "dl0", N, C, H, W)
+        call("wsl_s2l_head_bwd", probs, label, ulab, st, self.ctrl, S, N, C, H, W, d, d16, ex.dt)
+        self.loss_parts = {"ce": st[0], "u": st[2], "u_labels": ulab}
+        return st[4], [dl0]
+
+    def __call__(self, image, scribble, weight):
+        """image fp32 [N,1,H,W], scribble uint8 [N,H,W] (4 = unlabelled), weight fp32 [N,H,W,4] (S2LLoader's batch).  Returns the
+        loss (0-dim device tensor): NaN after thr_iter when no unlabelled pixel clears thr_conf, as the reference."""
+        assert weight.is_cuda and weight.dtype == torch.float32 and tuple(weight.shape) == (image.shape[0],) + tuple(image.shape[2:]) + (4,)
+        w_u = 0.5 if self.iter_num >= self.thr_iter else 0.0
+        if w_u != self._w_u:
+            self.ctrl[1].fill_(w_u)
+            self._w_u = w_u
+        if self.graph_enabled:
+            if self._wstatic is None:
+                self._wstatic = torch.empty_like(weight)
+            assert self._wstatic.shape == weight.shape, "graph mode needs a fixed batch shape"
+            if self._wstatic.data_ptr() != weight.data_ptr():
+                self._wstatic.copy_(weight, non_blocking=True)
+            self._weight = self._wstatic
+        else:
+            self._weight = weight.contiguous()
+        return super().__call__(image, scribble)
+
+    @torch.no_grad()
+    def refresh(self, store, alpha=0.2, chunk=64, size=256, masks=None):
+        """Ensemble refresh of train_s2l.py:221-243 into ``store.weight_live``: for every training slice in dataset order,
+        zoom(order 0) to size x size, softmax(model(img)) in TRAIN mode at batch 1 (BatchNorm on that slice's own statistics,
+        running statistics updated once per slice, dropout on), zoom back (order 0) and w = alpha*p + (1-alpha)*w.
+
+        Here `chunk` slices run as ONE per-sample-BatchNorm forward (exactly what `chunk` batch-1 training forwards compute, the
+        running statistics updated in slice order across chunks); one kernel then does softmax at the back-zoom source pixel
+        and the EMA.  masks (tests): dropout keep masks {encoder block: uint8 [len(store), h, w, C]} for the whole pass."""
+        assert store.weight_live is not None, "the store has no prediction memory (SliceStore.from_arrays(..., scribbles=))"
+        self.model.train()
+        n, dev = len(store), store.images.device
+        a, b = float(alpha), float(1.0 - alpha)
+        for s in range(0, n, int(chunk)):
+            idx = list(range(s, min(n, s + int(chunk))))
+            B = len(idx)
+            tab = store.table(idx, [(0, 0, 0, 0, 0)] * B)          # mode 0: zoom(order 0) only (:223-224)
+            img = torch.empty(B, 1, size, size, dtype=torch.float32, device=dev)
+            lab = torch.empty(B, size, size, dtype=torch.uint8, device=dev)
+            call("wsl_augment_batch", store.images, store.labels, tab, B, size, size, img, lab)
+            mk = None if masks is None else {k: v[s: s + B] for k, v in masks.items()}
+            outs, _ = self.ex.forward(img, True, False, mk, None, bn_per_sample=True)
+            max_hw = int(max(int(store.shapes[i, 0]) * int(store.shapes[i, 1]) for i in idx))
+            call("wsl_s2l_refresh", outs[0], tab, B, size, max_hw, a, b, store.weight_live)

@@ -216,6 +216,7 @@ class UNetExecutor:
         self._stat_bufs = {}
         self._stat_rows = ctypes.c_int(0)
         self._accumulate = False
+        self._bn_per_sample = False      # forward(..., bn_per_sample=True) is running
         self.stats = {"launches": 0}
 
     # ---------------------------------------------------------------- buffers
@@ -478,6 +479,18 @@ class UNetExecutor:
         save = self.buf(slot, tag + ".save", (2 * C,), torch.float32)
         ss = self.buf(slot, tag + ".ss", (2 * C,), torch.float32)
         deferred = stats_done if isinstance(stats_done, tuple) else None
+        if training and self._bn_per_sample:
+            # every image normalised by its own statistics (B batch-1 training forwards); {scale, shift} per image
+            save = self.buf(slot, tag + ".save_ps", (N, 2 * C), torch.float32)
+            ss = self.buf(slot, tag + ".ss_ps", (N, 2 * C), torch.float32)
+            call("wsl_bn_stats_ps", y, self.dt, N, H * W, C, bn.weight, bn.bias, bn.running_mean, bn.running_var,
+                 bn.num_batches_tracked, float(bn.momentum), float(bn.eps), save, ss, self._ws("bn_ps"))
+            p = L.drop_p
+            self._tag_bytes("bn_act", L, N * H * W * C * (4 if self.dt == 1 else 2) * (2.25 if pooled is not None else 2.0))
+            call("wsl_bn_act_fwd_ps", y, self.dt, ss, N, H, W, C, LRELU_SLOPE, p, mask, self._layer_seed(L),
+                 self.seed_dev if mask is None and p > 0 else None, act, pooled, pool_idx)
+            self._untag()
+            return save, ss
         if training and stats_done:
             pass                       # save / ss come from the convolution epilogue's partial rows (bn_finalize, or folded in below)
         elif training and self.sync_bn is not None:
@@ -597,8 +610,19 @@ class UNetExecutor:
                 pk["bias"][: L.Cout].copy_(L.conv.bias.detach())
 
     def forward(self, x: torch.Tensor, training: bool, need_grad: bool, masks: Optional[dict] = None,
-                chan_keep: Optional[list] = None, defer_join: bool = False):
-        """x: fp32 [N, in_chns, H, W] CUDA.  Returns (list of fp32 NCHW logits, slot)."""
+                chan_keep: Optional[list] = None, defer_join: bool = False, bn_per_sample: bool = False):
+        """x: fp32 [N, in_chns, H, W] CUDA.  Returns (list of fp32 NCHW logits, slot).
+
+        bn_per_sample (training, no gradient): compute exactly what N batch-1 training forwards compute -- every BatchNorm
+        normalises each image by that image's own statistics and the running statistics take the N updates in batch order
+        (the ensemble refresh of train_s2l.py:221-228 runs the model on one slice at a time in train mode)."""
+        if bn_per_sample:
+            assert training and not need_grad, "bn_per_sample is a training-mode forward without gradient"
+            self._bn_per_sample = True
+            try:
+                return self.forward(x, training, need_grad, masks, chan_keep, defer_join)
+            finally:
+                self._bn_per_sample = False
         assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4, "input must be a CUDA fp32 NCHW tensor"
         assert x.shape[1] == self.in_chns == 1, "executor is specialised to single-channel inputs (ACDC slices)"
         N, _, H, W = x.shape
@@ -622,9 +646,10 @@ class UNetExecutor:
             a1 = self.buf(slot, tag + ".a1", (N, h, w, C))
             y2 = self.buf(slot, tag + ".y2", (N, h, w, C))
             a2 = self.buf(slot, tag + ".a2", (N, h, w, C))
-            r1 = self.conv_fwd(l1, srcs, y1, 0, N, h, w, C, src_f32, bn_out=self.bn_bufs(l1, slot, tag + ".bn1") if training else None)
+            stats_in_conv = training and not self._bn_per_sample    # the conv epilogue's statistics are batch-wide
+            r1 = self.conv_fwd(l1, srcs, y1, 0, N, h, w, C, src_f32, bn_out=self.bn_bufs(l1, slot, tag + ".bn1") if stats_in_conv else None)
             sv1, ss1 = self.bn_fwd(l1, y1, a1, N, h, w, training, slot, tag + ".bn1", mask, stats_done=r1)
-            r2 = self.conv_fwd(l2, [a1], y2, 0, N, h, w, C, bn_out=self.bn_bufs(l2, slot, tag + ".bn2") if training else None)
+            r2 = self.conv_fwd(l2, [a1], y2, 0, N, h, w, C, bn_out=self.bn_bufs(l2, slot, tag + ".bn2") if stats_in_conv else None)
             pooled = idx = None
             if pool:
                 pooled = self.buf(slot, tag + ".pool", (N, h // 2, w // 2, C))
