@@ -185,7 +185,8 @@ int wsl_conv_tc(const void* src0, int C0, const void* src1, int C1, const void* 
                 void* out, int out_mode, int N, int H, int W, int CoutP, int CoutStore, int ksize, int dtype,
                 cudaStream_t stream);
 /* v2 of the same convolution: persistent CTAs, weights resident in shared memory, one halo load per pixel tile whose
- * nine taps are row-shifted wgmma descriptor views (no reload).  Same contract; needs W % 8 == 0 and H % 16 == 0. */
+ * nine taps are row-shifted wgmma descriptor views (no reload).  Same contract, except that out_mode must be 0 (16-bit NHWC)
+ * or 1 (fp32 NCHW); needs W % 8 == 0 and H % 16 == 0. */
 int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, const void* wpk_bf16, const float* bias,
                  void* out, int out_mode, int N, int H, int W, int CoutP, int CoutStore, int ksize, int dtype,
                  float* stat_partials, int* stat_rows_host, cudaStream_t stream);

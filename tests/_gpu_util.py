@@ -30,6 +30,29 @@ def chan_masks(seed, n):
 ENC_MASK_KEYS = ["encoder.in_conv.conv_conv.3"] + [f"encoder.down{i}.maxpool_conv.1.conv_conv.3" for i in range(1, 5)]
 
 
+def pack_conv_weights(w, c_slices, dt=0):
+    """Packed operands of a torch-layout weight w [Cout, Cin, k, k] on the GPU: 'wf' / 'bf' the forward packs (fp32 / 16-bit,
+    dt 0 = bf16, 2 = fp16 bits), 'wd' / 'bd' the data-gradient packs per input-channel slice in c_slices."""
+    from wsl4mis_b200._lib import call
+    dev = w.device
+    Cout, Cin, ks, _ = w.shape
+    T = ks * ks
+    CoutP, CinP = (Cout + 15) // 16 * 16, (Cin + 15) // 16 * 16
+    pk = {"wf": torch.zeros(T * CinP * CoutP, device=dev), "bf": torch.zeros(T * CinP * CoutP, device=dev, dtype=torch.bfloat16),
+          "wd": [], "bd": [], "CoutP": CoutP, "CinP": CinP}
+    beg = 0
+    for i, c in enumerate(c_slices):
+        sp = (c + 15) // 16 * 16
+        wd = torch.zeros(T * CoutP * sp, device=dev)
+        bd = torch.zeros(T * CoutP * sp, device=dev, dtype=torch.bfloat16)
+        call("wsl_pack_conv_weights", w, Cout, Cin, ks, CoutP, CinP, beg, c, pk["wf"] if i == 0 else None, wd,
+             pk["bf"] if i == 0 else None, bd, dt)
+        pk["wd"].append(wd)
+        pk["bd"].append(bd)
+        beg += c
+    return pk
+
+
 def rel_l2(a, b):
     a, b = a.double().flatten(), b.double().flatten()
     return ((a - b).norm() / (b.norm() + 1e-30)).item()

@@ -6,7 +6,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from _gpu_util import bf16_round, nchw, nhwc, rel_l2
+from _gpu_util import bf16_round, nchw, nhwc, pack_conv_weights, rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -21,26 +21,6 @@ ULP = {0: 2 ** -8, 2: 2 ** -11}
 
 def r16(x, dt):
     return x.to(T16[dt]).float()
-
-
-def _pack(w, c_slices, dt=0):
-    """returns dict of packed operands for torch-layout weight w [Cout,Cin,k,k]"""
-    Cout, Cin, ks, _ = w.shape
-    T = ks * ks
-    CoutP, CinP = (Cout + 15) // 16 * 16, (Cin + 15) // 16 * 16
-    pk = {"wf": torch.zeros(T * CinP * CoutP, device=DEV), "bf": torch.zeros(T * CinP * CoutP, device=DEV, dtype=BF),
-          "wd": [], "bd": [], "CoutP": CoutP, "CinP": CinP}
-    beg = 0
-    for i, c in enumerate(c_slices):
-        sp = (c + 15) // 16 * 16
-        wd = torch.zeros(T * CoutP * sp, device=DEV)
-        bd = torch.zeros(T * CoutP * sp, device=DEV, dtype=BF)
-        call("wsl_pack_conv_weights", w, Cout, Cin, ks, CoutP, CinP, beg, c, pk["wf"] if i == 0 else None, wd,
-             pk["bf"] if i == 0 else None, bd, dt)
-        pk["wd"].append(wd)
-        pk["bd"].append(bd)
-        beg += c
-    return pk
 
 
 CONV_CASES = [
@@ -75,7 +55,7 @@ def test_conv_forward(case, path):
     w = torch.randn(Cout, C0 + C1, ks, ks, generator=g) / np.sqrt((C0 + C1) * ks * ks)
     b = torch.randn(Cout, generator=g) * 0.1
     xin = torch.cat([x0, x1], 1) if C1 else x0
-    pk = _pack(w.to(DEV), [C0, C1] if C1 else [C0], dt)
+    pk = pack_conv_weights(w.to(DEV), [C0, C1] if C1 else [C0], dt)
     CoutP = pk["CoutP"]
     bias = torch.zeros(CoutP, device=DEV)
     bias[:Cout] = b.to(DEV)
@@ -125,7 +105,7 @@ def test_conv_dgrad(case, path):
     CoutP = (Cout + 15) // 16 * 16
     dy = torch.zeros(N, CoutP, H, W)
     dy[:, :Cout] = r16(torch.randn(N, Cout, H, W, generator=g), dt)
-    pk = _pack(w.to(DEV), [C0, C1] if C1 else [C0], dt)
+    pk = pack_conv_weights(w.to(DEV), [C0, C1] if C1 else [C0], dt)
     dyd = nhwc(dy, T16[dt]).to(DEV)
     wr = r16(w, dt) if path != "direct" else w
     ref = F.conv_transpose2d(dy[:, :Cout].double(), wr.double(), padding=ks // 2).float()
@@ -562,7 +542,7 @@ def test_dilated_convolution(dil, dt):
     w = torch.randn(Cout, C, ks, ks, generator=g) / np.sqrt(C * 9)
     b = torch.randn(Cout, generator=g) * 0.1
     dy = r16(torch.randn(N, Cout, H, W, generator=g), dt)
-    pk = _pack(w.to(DEV), [C], dt)
+    pk = pack_conv_weights(w.to(DEV), [C], dt)
     xd, dyd = nhwc(x, T16[dt]).to(DEV), nhwc(dy, T16[dt]).to(DEV)
     out = torch.zeros((N, H, W, Cout), device=DEV, dtype=T16[dt])
     call("wsl_conv_tc_dil", xd, C, None, 0, pk["bf"], b.to(DEV), out, 0, N, H, W, Cout, Cout, ks, dt, dil)

@@ -1615,6 +1615,8 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
                          int* stat_rows_host, cudaStream_t stream) {
   WSL_REQUIRE(ksize == 3 || ksize == 1, "wsl_conv_tc2: ksize must be 1 or 3");
   WSL_REQUIRE(dtype == 0 || dtype == 2, "wsl_conv_tc2: dtype must be 0 (bf16) or 2 (fp16)");
+  // both epilogues store 16-bit NHWC or fp32 NCHW only (store_pair(..., out_mode == 0 ? 0 : 1, ...))
+  WSL_REQUIRE(out_mode == 0 || out_mode == 1, "wsl_conv_tc2: out_mode must be 0 (16-bit NHWC) or 1 (fp32 NCHW), got %d", out_mode);
   WSL_REQUIRE(C0 % 16 == 0 && C1 % 16 == 0 && C0 > 0, "wsl_conv_tc2: source channels must be multiples of 16 (got %d,%d)", C0, C1);
   WSL_REQUIRE(CoutP % 16 == 0, "wsl_conv_tc2: CoutP must be a multiple of 16");
   {   // narrow outputs at >= 128-pixel rows: the row kernel (filter rows in N) is 1.8-2.3x faster per pixel

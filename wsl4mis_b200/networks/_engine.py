@@ -247,7 +247,8 @@ class UNetExecutor:
         return workspace(tag + ("" if not self._side_stack else "." + self._side_stack[-1]), self.dev)
 
     def _wgrad_partials(self):
-        """per-stream workspace for the split-K partial tiles of the deterministic weight gradient (largest layer: 144 CTAs x 196 KB)"""
+        """per-stream workspace for the split-K partial tiles of the deterministic weight gradient: the kernels launch about two CTAs
+        per SM with at most 3 x 64 x 128 floats (96 KB) each, about 25 MB of the 32 MB on a 132-SM H100"""
         key = ("wgp", self._side_stack[-1] if self._side_stack else "main")
         t = self._bufs.get(key)
         if t is None or t.device != self.dev:
