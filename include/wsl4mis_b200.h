@@ -155,6 +155,24 @@ int wsl_augment_batch_s2l(const float* images, const uint8_t* scribbles, const f
 int wsl_s2l_refresh(const float* logits, const void* table, int B, int S, long long max_hw, float alpha, float one_minus_alpha,
                     float* weights, cudaStream_t stream);
 
+/* Random-walker pseudo labels (dataloaders/acdc_pseudo_label_random_walker.py:9-26, pseudo_label_generator_acdc, and the per-slice
+ * loop :50-55; skimage random_walker(rescale_intensity(image, (-0.35, 1.35), (-1, 1)), markers, beta, mode='bf')) for n_slices
+ * ragged slices of a resident store (fp32 images and u8 scribbles at element offs[s], shapes[s] = {h, w}; scribble 0..3 = class,
+ * 4 = unlabelled).  A slice lacking a scribble of class 1, 2 or 3 gets all-zero labels and probabilities (:12-13).  Otherwise one
+ * persistent CTA solves L_UU x_l = -L_UM m_l for every label column by Jacobi-preconditioned CG (fp32 vectors, fp64 dot products
+ * in a fixed order) until max_l ||r_l|| / ||b_l|| <= tol or max_iter iterations; labels = argmax (seeds keep theirs), written as
+ * the pseudo label (label - 1, markers renumbered by rank when the background scribble is missing: DESIGN F17).  Slices are taken
+ * in the order given by `order` (descending pixel count keeps the last wave short).  probs ([px, 4] fp32, may be NULL) holds the
+ * per-column probabilities; iters / resid ([n_slices], indexed by slice id) the iteration count and final relative residual
+ * (iters = -1: the slice does not fit slot_px).  Results are bit-identical run to run and independent of the other slices.
+ * ws: caller-owned, wsl_random_walker_workspace() floats for `ctas` CTAs and slices of at most slot_px pixels (no zeroing needed).
+ * wsl_random_walker_workspace: ctas <= 0 picks the resident CTA count of the device; out2 is a HOST pointer receiving
+ * {ctas, workspace floats}. */
+int wsl_random_walker_workspace(int ctas, long long max_px, long long* out2);
+int wsl_random_walker(const float* images, const uint8_t* scribbles, const long long* offs, const int* shapes, const int* order,
+                      int n_slices, float beta, float tol, int max_iter, float* ws, int ctas, long long slot_px, uint8_t* labels,
+                      float* probs, int* iters, float* resid, cudaStream_t stream);
+
 /* ---- network operators (networks/unet.py) ---------------------------------------------------------------- */
 
 /* nn.Conv2d(k=3,pad=1)/(k=1) forward on CUDA cores (unet.py:19,23,55,120); with dgrad-packed weights also the

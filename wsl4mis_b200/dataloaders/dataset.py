@@ -256,7 +256,10 @@ class BaseDataSets(torch.utils.data.Dataset):
 
     base_dir: the ACDC directory (``ACDC_training_slices/*.h5`` with datasets image / label / scribble and
     ``ACDC_training_volumes/*.h5``; needs h5py), or ``'synthetic'`` / ``'synthetic:<patients>'`` for the deterministic
-    ACDC-shaped generator above (what the tests and benchmarks use: the GPU boxes have neither h5py nor the data)."""
+    ACDC-shaped generator above (what the tests and benchmarks use: the GPU boxes have neither h5py nor the data).
+
+    sup_type='random_walker' (train_weakly_supervised_pCE_random_walker_2D.py): slices without a 'random_walker' dataset get the
+    random-walker pseudo labels of their scribbles, computed on the GPU at construction (needs a CUDA device; no fallback)."""
 
     def __init__(self, base_dir=None, split='train', transform=None, fold="fold1", sup_type="label", num=None):
         self._base_dir, self.split, self.transform, self.sup_type = base_dir, split, transform, sup_type
@@ -279,13 +282,50 @@ class BaseDataSets(torch.utils.data.Dataset):
             self.sample_list = [f for f in names if f.split("_")[0] in ids]
         if num is not None and split == "train":
             self.sample_list = self.sample_list[:num]
+        self._rw = {}
+        if sup_type == "random_walker" and split == "train":
+            self._rw = self._random_walker_cache()
 
     def __len__(self):
         return len(self.sample_list)
 
+    def _random_walker_cache(self):
+        """{case: pseudo label} for the training slices whose source has no 'random_walker' dataset (the synthetic stand-in and the
+        shipped ACDC slice files, which hold only image / label / scribble).  The labels of the reference's offline generator
+        (acdc_pseudo_label_random_walker.py:9-26) are computed once, on the GPU, in this process (`random_walker_labels`) and kept
+        on the host: DataLoader workers read them without touching the GPU.  Files that do carry the dataset are read as before."""
+        todo, ims, scrs = [], [], []
+        for case in self.sample_list:
+            if self._synthetic is not None:
+                img, _, scr = self._synthetic[case.split("_")[0]]
+                z = int(case.rsplit("_", 1)[1].split(".")[0])
+                img, scr = img[z], scr[z]
+            else:
+                import h5py
+                with h5py.File(os.path.join(self._base_dir, "ACDC_training_slices", case), "r") as f:
+                    if "random_walker" in f:
+                        continue
+                    img, scr = f["image"][:], f["scribble"][:]
+            todo.append(case)
+            ims.append(np.asarray(img, np.float32))
+            scrs.append(np.asarray(scr).astype(np.uint8))
+        if not todo:
+            return {}
+        from .random_walker import random_walker_labels
+        labels, _ = random_walker_labels(ims, scrs, names=todo)
+        return dict(zip(todo, labels))
+
     def _read(self, case):
         """-> (image, label) numpy arrays of one train slice / one validation volume"""
         key = self.sup_type if self.split == "train" else "label"
+        if case in self._rw:
+            if self._synthetic is not None:
+                img = self._synthetic[case.split("_")[0]][0][int(case.rsplit("_", 1)[1].split(".")[0])]
+            else:
+                import h5py
+                with h5py.File(os.path.join(self._base_dir, "ACDC_training_slices", case), "r") as f:
+                    img = f["image"][:]
+            return img, self._rw[case]
         if self._synthetic is not None:
             img, lab, scr = self._synthetic[case.split("_")[0]]
             if self.split == "train":

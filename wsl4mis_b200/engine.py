@@ -8,6 +8,8 @@
   dmpls          train_weakly_supervised_segmentation_pCE_ours_proposed.py:108-132
   pce_entropy    train_weakly_supervised_pCE_Entropy_Mini_2D.py:97-109
   pce_variance   train_weakly_supervised_pCE_Inter&Intra_Class_2D.py:112-125 (weight = consistency * sigmoid_rampup(it//150, 200))
+  ce_dice        train_fully_supervised_2D.py:97-105 and train_weakly_supervised_pCE_random_walker_2D.py:97-104
+                 (0.5 * (CE(ignore_index=4) + DiceLoss(softmax, label)) on dense or random-walker labels)
 (``S2LStep`` below adds Scribble2Label, train_s2l.py:119-157, and its ensemble refresh :214-243) as ONE launch sequence: executor forward -> fused loss head (softmax+pCE, regulariser, combined backward into
 dlogits) -> executor backward into a flat fp32 gradient bucket -> (NCCL all-reduce of that bucket when
 world_size > 1) -> fused SGD(momentum 0.9, wd 1e-4) over the flat parameter buffer with the poly LR read from
@@ -28,7 +30,7 @@ from . import ddp
 from . import _lib
 from ._lib import call, workspace
 
-VARIANTS = ("pce", "pce_gatedcrf", "pce_ms", "pce_tv", "dmpls", "pce_entropy", "pce_variance")
+VARIANTS = ("pce", "pce_gatedcrf", "pce_ms", "pce_tv", "dmpls", "pce_entropy", "pce_variance", "ce_dice")
 
 
 class TrainStep:
@@ -138,6 +140,8 @@ class TrainStep:
         v = self.variant
         if self.global_batch and v in ("pce_tv", "pce_variance"):
             raise NotImplementedError(f"global_batch semantics are not defined here for '{v}' (batch-slice TV / per-sample variance ramps)")
+        if self.global_batch and v == "ce_dice":
+            raise NotImplementedError("global_batch semantics are not defined here for 'ce_dice' (run it with per-rank normalisers)")
         heads = range(self.n_heads_trained)
         probs, stats = [], []
         for h in heads:
@@ -205,6 +209,17 @@ class TrainStep:
             loss = ce + self.cw_dev[0] * out[0]
             d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
             call("wsl_head_bwd", probs[0], label, stats[0], None, 1.0 * S, gp, float(w) * S, N, C, H, W, 4, d, d16, self.ex.dt)
+        elif v == "ce_dice":
+            # DiceLoss(4)(softmax, label) has no ignore mask and no F14 weighting: pDLoss kernels with msum = NULL, mconst = 1
+            # (a label-4 pixel is in no class but its probabilities still enter the Z sums, as one_hot(4) does in the reference)
+            sums = B("dice0", (13,))
+            call("wsl_pdice_fwd", probs[0], label, None, 1.0, N, C, H, W, sums, workspace("pdice", dev))
+            gp = B("gprobs0", (N, C, H, W))
+            call("wsl_pdice_bwd", probs[0], label, None, 1.0, sums, N, C, H, W, 0.5, 0, gp)
+            loss = 0.5 * (ce + sums[0])
+            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
+            call("wsl_head_bwd", probs[0], label, stats[0], None, 0.5 * S, gp, 1.0 * S, N, C, H, W, 4, d, d16, self.ex.dt)
+            self.loss_parts = {"ce": ce, "dice": sums[0]}
         else:  # dmpls
             pseudo = B("pseudo", (N, H, W), torch.uint8)
             call("wsl_mix_argmax", probs[0], probs[1], 0.0, 0.0, self.beta_dev, N, C, H, W, pseudo)   # beta from device memory
