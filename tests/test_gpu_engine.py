@@ -175,7 +175,7 @@ def test_uamt_graph_replay_equals_eager():
         steps[graph].iter_num = 297
     worst = _lockstep(steps[False], steps[True], [((img_l, lab_l, img_u), {})] * 6, ("flat", "mom"))
     e, c = steps[False], steps[True]
-    assert c._graph is not None and c.launches_per_step > 500 and c.iter_num == e.iter_num == 303
+    assert list(c._graphs) == [0] and c.launches_per_step > 500 and c.iter_num == e.iter_num == 303
     assert e.parts["weight"] == c.parts["weight"] and e.parts["threshold"] == c.parts["threshold"]
     w0 = 0.1 * c.ramps.sigmoid_rampup(0, 200.0)
     assert c.parts["weight"] != w0                    # the ramp weight changed at iteration 300, inside the captured steps

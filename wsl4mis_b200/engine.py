@@ -33,7 +33,157 @@ from ._lib import call, workspace
 VARIANTS = ("pce", "pce_gatedcrf", "pce_ms", "pce_tv", "dmpls", "pce_entropy", "pce_variance", "ce_dice")
 
 
-class TrainStep:
+def _flatten(params, dev):
+    """One fp32 buffer holding `params` back to back, each p.data re-pointed into it (views keep the nn.Parameter objects /
+    state_dict intact) -> (buffer, {id(p): (offset, numel)})."""
+    flat = torch.empty(sum(p.numel() for p in params), dtype=torch.float32, device=dev)
+    offsets, off = {}, 0
+    for p in params:
+        flat[off:off + p.numel()].copy_(p.data.reshape(-1))
+        p.data = flat[off:off + p.numel()].view_as(p)
+        offsets[id(p)] = (off, p.numel())
+        off += p.numel()
+    return flat, offsets
+
+
+def _captured(fn):
+    """fn() captured into a new CUDA graph -> (graph, what fn returned)"""
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        out = fn()
+    return g, out
+
+
+class _FlatSGDStep:
+    """What every step class shares: the flat fp32 master parameters, the fused SGD over the trained `segments` of that buffer
+    with the poly LR read from device memory, and the driver `_run` that executes the subclass's
+    `_fwd_bwd(*inputs, **kw) -> (loss, flat gradient bucket)`, the all-reduce and `_finish` eagerly or as captured CUDA graphs.
+
+    Graph mode keeps `input_sets` sets of static input buffers (``input_buffers(i)``).  With two, a caller can copy batch k+1
+    from pinned host memory on a copy stream while the graph of batch k runs (bench.py's end-to-end leg does).  Tensors that are
+    not one of those buffers are copied into set 0.  After two eager warm-up steps one graph is captured per input set, or per
+    host key for a step that passes one (such a step keeps a single input set), and replayed from then on."""
+    aliases = ()            # attributes _fwd_bwd sets that alias graph memory: kept per graph and restored on every replay
+    input_sets = 2
+    nccl_in_graph = False   # world_size > 1: capture the all-reduce in the step graph instead of issuing it between two graphs
+
+    def __init__(self, model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group):
+        self.model, self.ex = model, model.executor
+        self.base_lr, self.max_iterations = float(base_lr), int(max_iterations)
+        self.momentum, self.weight_decay = float(momentum), float(weight_decay)
+        self.graph_enabled = bool(graph)
+        self.world_size, self.pg = int(world_size), process_group
+        self.iter_num = 0
+        self.dev = next(model.parameters()).device
+        self.flat, self.offsets = _flatten(self.ex.params, self.dev)
+        if self.world_size > 1:
+            ddp.broadcast_flat(self.flat, 0, self.pg)     # identical replicas (DDP does the same at construction)
+        self.mom = torch.zeros_like(self.flat)
+        self.lr_dev = torch.full((1,), self.base_lr, dtype=torch.float32, device=self.dev)
+        self.launches_per_step = 0
+        self._warm, self._graphs, self._static = 0, {}, [None] * self.input_sets
+
+    def _opt(self, g):
+        for off, n in self.segments:
+            call("wsl_sgd_step", self.flat[off:], g[off:], self.mom[off:], n, self.lr_dev, self.base_lr, self.momentum,
+                 self.weight_decay, 1.0 / self.world_size)
+
+    def _allreduce(self, g):
+        """sum the trained prefix of the bucket over the ranks (the SGD kernel applies the 1/world mean)"""
+        if self.world_size > 1:
+            ddp.allreduce_flat(g[: self.n_trained], self.pg)
+
+    def _finish(self, g, captured):
+        """the update after the all-reduce.  captured: it runs inside a graph, so host values must reach it through device memory"""
+        self._opt(g)
+
+    def _step(self, inputs, kw, captured):
+        loss, g = self._fwd_bwd(*inputs, **kw)
+        self._allreduce(g)
+        self._finish(g, captured)
+        return loss, g
+
+    def _advance_lr(self):
+        # poly LR applied after the step with the pre-increment iteration (...pCE_2D.py:106-108)
+        self.lr_dev.fill_(self.base_lr * (1.0 - self.iter_num / self.max_iterations) ** 0.9)
+        self.iter_num += 1
+
+    def _run(self, inputs, key=None, **kw):
+        """One training step on `inputs` (the tensors `_fwd_bwd` reads; kw: its host arguments).  `key` names the host values a
+        captured graph bakes in (USTM's rot90 count); without one, graphs are keyed by input set.  Returns the loss (0-dim device
+        tensor)."""
+        if self.graph_enabled:
+            s = 0
+            for i, st in enumerate(self._static):
+                if st is not None and st[0].data_ptr() == inputs[0].data_ptr():
+                    s = i
+            static = self.input_buffers(s, like=inputs)
+            for buf, x in zip(static, inputs):
+                assert buf.shape == x.shape, "graph mode needs a fixed batch shape"
+                if buf.data_ptr() != x.data_ptr():
+                    buf.copy_(x, non_blocking=True)
+            inputs = static
+        if not self.graph_enabled or self._warm < 2:       # graph mode: the eager warm-up allocates every buffer / tensor map
+            c0 = _lib.COUNTERS["launch_calls"]
+            loss, _ = self._step(inputs, kw, False)
+            self.launches_per_step = _lib.COUNTERS["launch_calls"] - c0
+            self._warm += 1
+        else:
+            k = s if key is None else key
+            if k not in self._graphs:
+                self._graphs[k] = self._capture(inputs, kw) + (tuple(getattr(self, a) for a in self.aliases),)
+            g1, g2, gloss, gg, kept = self._graphs[k]
+            for a, v in zip(self.aliases, kept):
+                setattr(self, a, v)
+            g1.replay()
+            if g2 is not None:                  # two-graph mode: the all-reduce is issued from the host between the graphs
+                self._allreduce(gg)
+                g2.replay()
+            # the captured loss lives in graph-pool memory that the next replay overwrites: hand out a copy
+            # (the aliased attributes, e.g. step.outputs, still point into the pool: read them before the next step)
+            loss = gloss.clone()
+        self._advance_lr()
+        return loss
+
+    def _capture(self, inputs, kw):
+        """Capture the step -> (graph, second graph or None, loss, gradient bucket).  world_size 1: one graph.  world_size > 1
+        with nccl_in_graph: ONE graph as well, with the all-reduces captured inside it (no host round trip and no second graph
+        launch between backward and optimiser); otherwise, or if this NCCL / torch build refuses to capture the collective, two
+        graphs (forward+backward | update) with the all-reduce issued from the host in between."""
+        torch.cuda.synchronize()
+        if self.world_size > 1 and self.nccl_in_graph:
+            try:
+                g1, (gloss, gg) = _captured(lambda: self._step(inputs, kw, True))
+                self.comm_mode = "captured in the step graph (decoder slice overlapped with the encoder backward)" if self.overlap_comm else "captured in the step graph"
+                return g1, None, gloss, gg
+            except Exception as e:                   # pragma: no cover - depends on the NCCL build
+                self.comm_mode = f"two graphs, host-issued all-reduce (capture failed: {type(e).__name__})"
+                torch.cuda.synchronize()
+                self.overlap_comm = False            # a host-issued collective cannot sit inside backward()
+        if self.world_size == 1:
+            g1, (gloss, gg) = _captured(lambda: self._step(inputs, kw, True))
+            return g1, None, gloss, gg
+        if not hasattr(self, "comm_mode"):
+            self.comm_mode = "two graphs, host-issued all-reduce"
+        g1, (gloss, gg) = _captured(lambda: self._fwd_bwd(*inputs, **kw))
+        g2, _ = _captured(lambda: self._finish(gg, True))
+        return g1, g2, gloss, gg
+
+    def input_buffers(self, idx=0, like=None):
+        """The device buffers read by the graphs of input set `idx` (0 .. input_sets - 1), one per tensor the step takes."""
+        if self._static[idx] is None:
+            src = like if like is not None else next((st for st in self._static if st is not None), None)
+            assert src is not None, "call the step once (or pass like=) before asking for input buffers"
+            self._static[idx] = tuple(torch.empty_like(t) for t in src)
+        return self._static[idx]
+
+    def static_inputs(self):
+        return self._static[0]
+
+
+class TrainStep(_FlatSGDStep):
+    aliases = ("_outs", "loss_parts")
+
     def __init__(self, model, variant="pce_gatedcrf", base_lr=0.01, max_iterations=30000, momentum=0.9,
                  weight_decay=1e-4, graph=True, process_group=None, world_size=1, global_batch=False):
         """global_batch (world_size > 1): reproduce the SINGLE-PROCESS arithmetic of the reference at the global batch (SURVEY 8(e)):
@@ -42,38 +192,13 @@ class TrainStep:
         and loss normalisers), which is what the weak-scaling benchmark runs.  The collectives are issued from the host inside the
         step, so this mode runs eagerly (no CUDA graph)."""
         assert variant in VARIANTS
-        self.model, self.variant = model, variant
-        self.ex = model.executor
-        self.base_lr, self.max_iterations = float(base_lr), int(max_iterations)
-        self.momentum, self.weight_decay = float(momentum), float(weight_decay)
-        self.graph_enabled = bool(graph)
-        self.world_size = int(world_size)
-        self.pg = process_group
+        super().__init__(model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group)
+        self.variant = variant
         self.global_batch = bool(global_batch) and self.world_size > 1
         if self.global_batch:
             self.graph_enabled = False
             self.ex.sync_bn = (self.world_size, self.pg)
-        self.iter_num = 0
-        self._graphs = [None, None]
-        self._warm = 0
-        self._static = [None, None]
-        dev = next(model.parameters()).device
-        self.dev = dev
-        # flat fp32 master parameters (views keep the nn.Parameter objects / state_dict intact)
-        params = self.ex.params
-        n = sum(p.numel() for p in params)
-        self.flat = torch.empty(n, dtype=torch.float32, device=dev)
-        off = 0
-        self.offsets = {}
-        for p in params:
-            self.flat[off:off + p.numel()].copy_(p.data.reshape(-1))
-            p.data = self.flat[off:off + p.numel()].view_as(p)
-            self.offsets[id(p)] = (off, p.numel())
-            off += p.numel()
-        if self.world_size > 1:
-            ddp.broadcast_flat(self.flat, 0, self.pg)     # identical replicas (DDP does the same at construction)
-        self.mom = torch.zeros_like(self.flat)
-        self.lr_dev = torch.full((1,), self.base_lr, dtype=torch.float32, device=dev)
+        dev = self.dev
         self.beta_dev = torch.tensor([0.5, 0.5], dtype=torch.float32, device=dev)
         self.cw_dev = torch.zeros(1, dtype=torch.float32, device=dev)
         self.consistency, self.consistency_rampup = 0.1, 200.0
@@ -93,7 +218,7 @@ class TrainStep:
             skip.update(id(q) for q in self.model.aux_decoder1.parameters())
         skip.update(id(q) for nm, q in model.named_parameters() if "out_conv_dp" in nm)
         self.segments = []
-        for p in params:
+        for p in self.ex.params:
             if id(p) in skip or id(p) not in self.ex.used_param_ids:
                 continue
             off_p, n_p = self.offsets[id(p)]
@@ -110,7 +235,6 @@ class TrainStep:
         if self.graph_enabled and not self.nccl_in_graph:
             self.overlap_comm = False        # a host-issued collective cannot sit inside the captured backward
         self.loss_parts = {}
-        self.launches_per_step = 0
 
     # ------------------------------------------------------------------
     @staticmethod
@@ -122,6 +246,14 @@ class TrainStep:
             return None, d16, ("nhwc16", d16)
         d = ex.buf(slot, "head." + name, (N, C, H, W), torch.float32)
         return d, None, d
+
+    def _head_bwd(self, h, probs, stats, label, ce_w, gp, reg_w, slot):
+        """head h's logit gradient ce_w * d(pCE) + reg_w * gp (gp: the regulariser's probability gradient or None), written by
+        wsl_head_bwd into a `_dlogits` buffer -> what backward() receives for that head"""
+        N, C, H, W = probs[h].shape
+        d, d16, dl = self._dlogits(self.ex, slot, f"dl{h}", N, C, H, W)
+        call("wsl_head_bwd", probs[h], label, stats[h], None, ce_w, gp, reg_w, N, C, H, W, 4, d, d16, self.ex.dt)
+        return dl
 
     def _head(self, logits_list, image, label, slot):
         """loss head: returns (loss tensor, [dlogits per decoder or None])."""
@@ -157,15 +289,13 @@ class TrainStep:
         ce = stats[0][0]
         if v == "pce":
             loss = ce
-            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
-            call("wsl_head_bwd", probs[0], label, stats[0], None, 1.0 * S, None, 0.0 * S, N, C, H, W, 4, d, d16, self.ex.dt)
+            dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, None, 0.0 * S, slot)
         elif v == "pce_gatedcrf":
             gp = B("gprobs0", (N, C, H, W))
             out = B("crf", (2,))
             call("wsl_gatedcrf_fwd", probs[0], image, gp, N, C, H, W, 5, 6.0, 0.1, 1.0, out, workspace("crf", dev))
             loss = ce + 0.1 * out[0]
-            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
-            call("wsl_head_bwd", probs[0], label, stats[0], None, 1.0 * S, gp, 0.1 * S * G, N, C, H, W, 4, d, d16, self.ex.dt)
+            dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, 0.1 * S * G, slot)
             self.loss_parts = {"ce": ce, "crf": out[0]}
         elif v == "pce_ms":
             gp = B("gprobs0", (N, C, H, W))
@@ -174,8 +304,7 @@ class TrainStep:
             call("wsl_mumford_shah_fwd", image, probs[0], N, C, H, W, out, cent, workspace("ms", dev))
             call("wsl_mumford_shah_bwd", image, probs[0], cent, N, C, H, W, 1e-6, 0, gp)
             loss = ce + 1e-6 * out[0]
-            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
-            call("wsl_head_bwd", probs[0], label, stats[0], None, 1.0 * S, gp, 1.0 * S, N, C, H, W, 4, d, d16, self.ex.dt)
+            dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, 1.0 * S, slot)
         elif v == "pce_tv":
             # tv_loss(outputs_soft[1:]) -- batch slice, sample 0 gets no TV term (SURVEY F12)
             gp = B("gprobs0", (N, C, H, W))
@@ -186,16 +315,14 @@ class TrainStep:
                 loss = ce + 1e-2 * out[0]
             else:
                 loss = ce   # mean over an empty tensor is NaN in the reference; N=1 is never used with this script
-            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
-            call("wsl_head_bwd", probs[0], label, stats[0], None, 1.0 * S, gp, 1.0 * S, N, C, H, W, 4, d, d16, self.ex.dt)
+            dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, 1.0 * S, slot)
         elif v == "pce_entropy":
             gp = B("gprobs0", (N, C, H, W))
             out = B("ent", (1,))
             call("wsl_entropy_fwd", probs[0], N, C, H, W, out, workspace("ent", dev))
             call("wsl_entropy_bwd", probs[0], N, C, H, W, 0.1, 0, gp)
             loss = ce + 0.1 * out[0]
-            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
-            call("wsl_head_bwd", probs[0], label, stats[0], None, 1.0 * S, gp, 1.0 * S * G, N, C, H, W, 4, d, d16, self.ex.dt)
+            dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, 1.0 * S * G, slot)
         elif v == "pce_variance":
             from .utils import ramps
             w = self.consistency * ramps.sigmoid_rampup(self.iter_num // 150, self.consistency_rampup)
@@ -207,8 +334,7 @@ class TrainStep:
             # the ramp weight changes every 150 iterations: it multiplies on the device side so graphs stay valid
             self.cw_dev.fill_(w)
             loss = ce + self.cw_dev[0] * out[0]
-            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
-            call("wsl_head_bwd", probs[0], label, stats[0], None, 1.0 * S, gp, float(w) * S, N, C, H, W, 4, d, d16, self.ex.dt)
+            dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, float(w) * S, slot)
         elif v == "ce_dice":
             # DiceLoss(4)(softmax, label) has no ignore mask and no F14 weighting: pDLoss kernels with msum = NULL, mconst = 1
             # (a label-4 pixel is in no class but its probabilities still enter the Z sums, as one_hot(4) does in the reference)
@@ -217,8 +343,7 @@ class TrainStep:
             gp = B("gprobs0", (N, C, H, W))
             call("wsl_pdice_bwd", probs[0], label, None, 1.0, sums, N, C, H, W, 0.5, 0, gp)
             loss = 0.5 * (ce + sums[0])
-            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
-            call("wsl_head_bwd", probs[0], label, stats[0], None, 0.5 * S, gp, 1.0 * S, N, C, H, W, 4, d, d16, self.ex.dt)
+            dl[0] = self._head_bwd(0, probs, stats, label, 0.5 * S, gp, 1.0 * S, slot)
             self.loss_parts = {"ce": ce, "dice": sums[0]}
         else:  # dmpls
             pseudo = B("pseudo", (N, H, W), torch.uint8)
@@ -237,13 +362,11 @@ class TrainStep:
                 gp = B(f"gprobs{h}", (N, C, H, W))
                 call("wsl_pdice_bwd", probs[h], pseudo, None, nb, sums, N, C, H, W, 0.25, 0, gp)
                 loss = loss + 0.25 * sums[0]
-                d, d16, dl[h] = self._dlogits(ex, slot, f"dl{h}", N, C, H, W)
-                call("wsl_head_bwd", probs[h], label, stats[h], None, 0.5 * S, gp, 1.0 * S, N, C, H, W, 4, d, d16, self.ex.dt)
+                dl[h] = self._head_bwd(h, probs, stats, label, 0.5 * S, gp, 1.0 * S, slot)
         return loss, dl
 
     def _fwd_bwd(self, image, label):
         ex = self.ex
-        c0 = _lib.COUNTERS["launch_calls"]
         # single-head scripts on the two-head model never read the aux output: let its forward keep running on the
         # side stream underneath the loss head and the main backward (joined at the end of the backward)
         defer = self.two_heads and self.n_heads_trained == 1
@@ -256,13 +379,7 @@ class TrainStep:
         finally:
             ex.on_decoders_done = None
         self._outs = outs
-        self.launches_per_step = _lib.COUNTERS["launch_calls"] - c0 + 1     # + the SGD kernel (also inside the graph)
         return loss, gflat
-
-    def _opt(self, gflat):
-        for off, n in self.segments:
-            call("wsl_sgd_step", self.flat[off:], gflat[off:], self.mom[off:], n, self.lr_dev, self.base_lr, self.momentum,
-                 self.weight_decay, 1.0 / self.world_size)
 
     def _allreduce_decoders(self, gflat):
         """called by the executor between the decoder and encoder halves of backward(): sum the decoder slice of the bucket on the
@@ -273,23 +390,19 @@ class TrainStep:
 
     def _allreduce(self, gflat):
         """the rest of the bucket after backward(): the encoder slice (or everything when the overlap is off)"""
-        if self.world_size > 1:
-            if self.overlap_comm:
-                # SAME stream as the decoder slice: two collectives of one communicator on different streams may be scheduled in
-                # different orders on different ranks (synchronous c10d collectives run on the caller's stream) and deadlock
-                with self.ex.on_side("comm"):
-                    ddp.allreduce_flat(gflat[: self.enc_end], self.pg)
-                self.ex.join_side("comm")
-            else:
-                ddp.allreduce_flat(gflat[: self.n_trained], self.pg)
+        if self.overlap_comm:
+            # SAME stream as the decoder slice: two collectives of one communicator on different streams may be scheduled in
+            # different orders on different ranks (synchronous c10d collectives run on the caller's stream) and deadlock
+            with self.ex.on_side("comm"):
+                ddp.allreduce_flat(gflat[: self.enc_end], self.pg)
+            self.ex.join_side("comm")
+        else:
+            super()._allreduce(gflat)
 
     # ------------------------------------------------------------------
     def __call__(self, image, label):
         """image: fp32 [N,1,H,W] CUDA, label: uint8 [N,H,W] CUDA.  Returns the loss (0-dim device tensor).
-
-        Graph mode keeps TWO sets of static input buffers (``input_buffers(0/1)``) with one captured graph each, so a
-        caller can copy batch k+1 from pinned host memory on a copy stream while the graph of batch k runs
-        (bench.py's end-to-end leg does).  Tensors that are not one of those buffers are copied into set 0."""
+        Graph mode: ``input_buffers(0/1)`` are (image, label) pairs (see `_FlatSGDStep`)."""
         assert image.is_cuda and label.is_cuda and label.dtype == torch.uint8
         self.model.train()
         if self.variant == "dmpls":
@@ -297,93 +410,14 @@ class TrainStep:
             # device memory so the captured graph sees a fresh value every replay
             self.beta = random.random() + 1e-10
             self.beta_dev.copy_(torch.tensor([self.beta, 1.0 - self.beta], dtype=torch.float32), non_blocking=False)
-        if not self.graph_enabled:
-            loss, g = self._fwd_bwd(image, label)
-            self._allreduce(g)
-            self._opt(g)
-        else:
-            idx = 0
-            for i, st in enumerate(self._static):
-                if st is not None and st[0].data_ptr() == image.data_ptr():
-                    idx = i
-            simg, slab = self.input_buffers(idx, like=(image, label))
-            assert simg.shape == image.shape, "graph mode needs a fixed batch shape"
-            if simg.data_ptr() != image.data_ptr():
-                simg.copy_(image, non_blocking=True)
-            if slab.data_ptr() != label.data_ptr():
-                slab.copy_(label, non_blocking=True)
-            if self._warm < 2:                      # eager warm-up allocates every buffer / tensor map
-                loss, g = self._fwd_bwd(simg, slab)
-                self._allreduce(g)
-                self._opt(g)
-                self._warm += 1
-            else:
-                if self._graphs[idx] is None:
-                    self._graphs[idx] = self._capture(simg, slab)
-                g1, g2, gloss, gg, self._outs, self.loss_parts = self._graphs[idx]
-                g1.replay()
-                if g2 is not None:                  # two-graph fallback: NCCL issued from the host between the graphs
-                    self._allreduce(gg)
-                    g2.replay()
-                # the captured loss lives in graph-pool memory that the next replay overwrites: hand out a copy
-                # (step.outputs / step.loss_parts still alias the pool: read them before the next step)
-                loss = gloss.clone()
-        # poly LR applied after the step with the pre-increment iteration (...pCE_2D.py:106-108)
-        lr_ = self.base_lr * (1.0 - self.iter_num / self.max_iterations) ** 0.9
-        self.lr_dev.fill_(lr_)
-        self.iter_num += 1
-        return loss
-
-    def _capture(self, simg, slab):
-        """Capture the step.  world_size 1: one graph.  world_size > 1: ONE graph as well, with the NCCL all-reduces captured
-        inside it (decoder slice on a side branch under the encoder's backward, encoder slice + SGD at the end) -- no host round
-        trip and no second graph launch between backward and optimiser; if this NCCL / torch build refuses to capture the
-        collective, fall back to two graphs with the all-reduce issued from the host in between."""
-        torch.cuda.synchronize()
-        if self.world_size > 1 and self.nccl_in_graph:
-            try:
-                g1 = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g1):
-                    gloss, gg = self._fwd_bwd(simg, slab)
-                    self._allreduce(gg)
-                    self._opt(gg)
-                self.comm_mode = "captured in the step graph (decoder slice overlapped with the encoder backward)" if self.overlap_comm else "captured in the step graph"
-                return (g1, None, gloss, gg, self._outs, dict(self.loss_parts))
-            except Exception as e:                   # pragma: no cover - depends on the NCCL build
-                self.comm_mode = f"two graphs, host-issued all-reduce (capture failed: {type(e).__name__})"
-                torch.cuda.synchronize()
-                self.overlap_comm = False            # a host-issued collective cannot sit inside backward()
-        g1 = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g1):
-            gloss, gg = self._fwd_bwd(simg, slab)
-            if self.world_size == 1:
-                self._opt(gg)
-        g2 = None
-        if self.world_size > 1:
-            if not hasattr(self, "comm_mode"):
-                self.comm_mode = "two graphs, host-issued all-reduce"
-            g2 = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g2):
-                self._opt(gg)
-        return (g1, g2, gloss, gg, self._outs, dict(self.loss_parts))
-
-    def input_buffers(self, idx=0, like=None):
-        """(image, label) device buffers read by captured graph `idx` (0 or 1)."""
-        if self._static[idx] is None:
-            src = like if like is not None else self._static[1 - idx]
-            assert src is not None, "call the step once (or pass like=) before asking for input buffers"
-            self._static[idx] = (torch.empty_like(src[0]), torch.empty_like(src[1]))
-        return self._static[idx]
-
-    def static_inputs(self):
-        return self._static[0]
+        return self._run((image, label))
 
     @property
     def outputs(self):
         return self._outs
 
 
-class UAMTStep:
+class UAMTStep(_FlatSGDStep):
     """Per-step body of train_uncertainty_aware_mean_teacher_2D.py:138-197 (BASELINE config 5) on the fused kernels.
 
     Batch = labelled half + unlabelled half.  Student: two training forwards with gradient (labelled, unlabelled);
@@ -391,6 +425,8 @@ class UAMTStep:
     noisy unlabelled inputs and T/2 = 4 no-grad forwards on the twice-repeated noisy batch (T = 8 stochastic passes).
     Loss = 0.5*(Dice + CE) on the labelled half + w(t) * uncertainty-masked softmax-MSE consistency (K13 kernels).
     Two-head models (unet_cct) use main_seg on both sides (SURVEY F7)."""
+    aliases = ("parts",)
+    input_sets = 1          # USTM keys its graphs by the rot90 count alone
 
     def __init__(self, model, ema_model, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0,
                  momentum=0.9, weight_decay=1e-4, T=8, process_group=None, world_size=1, graph=False):
@@ -404,38 +440,21 @@ class UAMTStep:
         weight :183, uncertainty threshold :186, poly LR :194) stay host arithmetic: they are written to a 2-float device buffer
         before every replay and read by the kernels through their *_ptr arguments.  Needs a fixed batch shape and noises=None."""
         from .utils import ramps
-        self.world_size, self.pg = int(world_size), process_group
+        super().__init__(model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group)
         self.ramps = ramps
-        self.model, self.ema_model = model, ema_model
-        self.ex, self.ex_t = model.executor, ema_model.executor
-        self.base_lr, self.max_iterations = float(base_lr), int(max_iterations)
+        self.ema_model, self.ex_t = ema_model, ema_model.executor
         self.consistency, self.consistency_rampup = float(consistency), float(consistency_rampup)
-        self.momentum, self.weight_decay, self.T = float(momentum), float(weight_decay), int(T)
-        self.iter_num = 0
-        dev = next(model.parameters()).device
-        self.dev = dev
-        params = self.ex.params
-        n = sum(p.numel() for p in params)
-        self.flat = torch.empty(n, dtype=torch.float32, device=dev)
-        off = 0
-        for p in params:
-            self.flat[off:off + p.numel()].copy_(p.data.reshape(-1))
-            p.data = self.flat[off:off + p.numel()].view_as(p)
-            off += p.numel()
+        self.T = int(T)
+        # the optimiser walks the prefix of the flat buffer in front of the first aux_decoder1 parameter
         first_aux = next(model.aux_decoder1.parameters()) if len(self.ex.dec) == 2 else None
-        self.n_trained = n if first_aux is None else sum(p.numel() for p in params[: [id(q) for q in params].index(id(first_aux))])
+        self.n_trained = self.flat.numel() if first_aux is None else self.offsets[id(first_aux)][0]
+        self.segments = [[0, self.n_trained]]
         if self.world_size > 1:
-            ddp.broadcast_flat(self.flat, 0, self.pg)
             for q in list(ema_model.parameters()) + list(ema_model.buffers()):
                 ddp.broadcast_flat(q.data, 0, self.pg)
-        self.mom = torch.zeros_like(self.flat)
-        self.lr_dev = torch.full((1,), self.base_lr, dtype=torch.float32, device=dev)
         from .networks._engine import initial_rng_counter
-        self.seed_dev = torch.full((1,), initial_rng_counter() ^ 0x5A5A5A5A, dtype=torch.int64, device=dev)
-        self.ramp_dev = torch.zeros(2, dtype=torch.float32, device=dev)            # {uncertainty threshold, consistency weight}
-        self.graph_enabled = bool(graph)
-        self._warm, self._graph, self._static = 0, None, None
-        self.launches_per_step = 0
+        self.seed_dev = torch.full((1,), initial_rng_counter() ^ 0x5A5A5A5A, dtype=torch.int64, device=self.dev)
+        self.ramp_dev = torch.zeros(2, dtype=torch.float32, device=self.dev)       # {uncertainty threshold, consistency weight}
 
     def _noisy(self, x, reps, salt, given):
         if given is not None:
@@ -443,6 +462,21 @@ class UAMTStep:
         out = torch.empty((x.shape[0] * reps,) + tuple(x.shape[1:]), dtype=torch.float32, device=self.dev)
         call("wsl_add_clamped_noise", x, x.numel(), reps, 0.1, 0.2, 0xA5A5 + salt, self.seed_dev, out)
         return out
+
+    def _teacher(self, img, noises):
+        """the teacher's no-grad passes on noisy copies of img: one at batch B -> ema_out, then T/2 on the twice-repeated batch
+        whose logits fill mc [T*B, C, H, W] in order.  noises (tests): the 1 + T/2 noise tensors; None draws them on the device"""
+        ex_t = self.ex_t
+        B, _, H, W = img.shape
+        tmasks, tck = getattr(self.ema_model, "dropout_masks", None), getattr(self.ema_model, "channel_keep", None)
+        ema_out = ex_t.forward(self._noisy(img, 1, 0, None if noises is None else noises[0]), True, False, tmasks, tck)[0][0]
+        mc = self.ex.buf("teacher", "mc", (self.T * B, 4, H, W), torch.float32)
+        for i in range(self.T // 2):
+            tm2 = None if tmasks is None else {k: v.repeat(2, 1, 1, 1) for k, v in tmasks.items()}
+            tck2 = None if tck is None else [c.repeat(2, 1) for c in tck]
+            lg = ex_t.forward(self._noisy(img, 2, 1 + i, None if noises is None else noises[1 + i]), True, False, tm2, tck2)[0][0]
+            mc[2 * B * i: 2 * B * (i + 1)].copy_(lg)
+        return ema_out, mc
 
     def _ramps(self):
         """host arithmetic of :183 and :186 for the current iteration -> (threshold, weight), also written to ramp_dev"""
@@ -452,82 +486,28 @@ class UAMTStep:
         self.ramp_dev.copy_(torch.tensor([thr, cw], dtype=torch.float32))
         return thr, cw
 
-    def _opt(self, g):
-        call("wsl_sgd_step", self.flat, g, self.mom, self.n_trained, self.lr_dev, self.base_lr, self.momentum, self.weight_decay,
-             1.0 / self.world_size)
-
     def __call__(self, image_l, label_l, image_u, noises=None):
         """image_l/image_u: fp32 [B,1,H,W]; label_l: uint8 [B,H,W] dense.  noises (tests): list of 1 + T/2 tensors holding
         the already-clamped noise of :147-149 and :167-169.  Returns the loss (0-dim device tensor)."""
         self.model.train()
         self.ema_model.train()
         thr, cw = self._ramps()
-        if not self.graph_enabled:
-            loss, g = self._body(image_l, label_l, image_u, noises)
-            if self.world_size > 1:
-                ddp.allreduce_flat(g[: self.n_trained], self.pg)
-            self._opt(g)
-        else:
-            assert noises is None, "graph mode draws the teacher noise on the device"
-            if self._static is None:
-                self._static = (torch.empty_like(image_l), torch.empty_like(label_l), torch.empty_like(image_u))
-            sl, sb, su = self._static
-            assert sl.shape == image_l.shape and su.shape == image_u.shape, "graph mode needs a fixed batch shape"
-            sl.copy_(image_l, non_blocking=True)
-            sb.copy_(label_l, non_blocking=True)
-            su.copy_(image_u, non_blocking=True)
-            if self._warm < 2:                      # eager warm-up allocates every buffer / tensor map / workspace
-                c0 = _lib.COUNTERS["launch_calls"]
-                loss, g = self._body(sl, sb, su, None)
-                if self.world_size > 1:
-                    ddp.allreduce_flat(g[: self.n_trained], self.pg)
-                self._opt(g)
-                self.launches_per_step = _lib.COUNTERS["launch_calls"] - c0
-                self._warm += 1
-            else:
-                if self._graph is None:
-                    torch.cuda.synchronize()
-                    g1, g2 = torch.cuda.CUDAGraph(), None
-                    with torch.cuda.graph(g1):
-                        gloss, gg = self._body(sl, sb, su, None)
-                        if self.world_size == 1:
-                            self._opt(gg)
-                    if self.world_size > 1:
-                        g2 = torch.cuda.CUDAGraph()
-                        with torch.cuda.graph(g2):
-                            self._opt(gg)
-                    self._graph = (g1, g2, gloss, gg, dict(self.parts))
-                    self.comm_mode = "two graphs, host-issued all-reduce"
-                g1, g2, gloss, gg, self.parts = self._graph
-                g1.replay()
-                if g2 is not None:
-                    ddp.allreduce_flat(gg[: self.n_trained], self.pg)
-                    g2.replay()
-                loss = gloss.clone()                # the captured loss lives in graph-pool memory
+        assert noises is None or not self.graph_enabled, "graph mode draws the teacher noise on the device"
+        loss = self._run((image_l, label_l, image_u), noises=noises)
         self.parts = dict(self.parts, weight=cw, threshold=thr)
-        lr_ = self.base_lr * (1.0 - self.iter_num / self.max_iterations) ** 0.9
-        self.lr_dev.fill_(lr_)
-        self.iter_num += 1
         return loss
 
-    def _body(self, image_l, label_l, image_u, noises):
+    def _fwd_bwd(self, image_l, label_l, image_u, noises=None):
         """forward passes, losses and both backward passes; returns (loss, flat gradient bucket)"""
-        ex, ex_t, dev = self.ex, self.ex_t, self.dev
+        ex, dev = self.ex, self.dev
         B, _, H, W = image_u.shape
         C, T = 4, self.T
         self.seed_dev.add_(1)
         masks, ck = getattr(self.model, "dropout_masks", None), getattr(self.model, "channel_keep", None)
-        tmasks, tck = getattr(self.ema_model, "dropout_masks", None), getattr(self.ema_model, "channel_keep", None)
         outs_l, slot_l = ex.forward(image_l.contiguous(), True, True, masks, ck)
         outs_u, slot_u = ex.forward(image_u.contiguous(), True, True, masks, ck)
         out_l, out_u = outs_l[0], outs_u[0]
-        ema_out = ex_t.forward(self._noisy(image_u, 1, 0, None if noises is None else noises[0]), True, False, tmasks, tck)[0][0]
-        mc = ex.buf("uamt", "mc", (T * B, C, H, W), torch.float32)
-        for i in range(T // 2):
-            tm2 = None if tmasks is None else {k: v.repeat(2, 1, 1, 1) for k, v in tmasks.items()}
-            tck2 = None if tck is None else [c.repeat(2, 1) for c in tck]
-            lg = ex_t.forward(self._noisy(image_u, 2, 1 + i, None if noises is None else noises[1 + i]), True, False, tm2, tck2)[0][0]
-            mc[2 * B * i: 2 * B * (i + 1)].copy_(lg)
+        ema_out, mc = self._teacher(image_u, noises)
         Bf = lambda name, shape, dt=torch.float32: ex.buf("uamt", name, shape, dt)
         # ---- supervised half: 0.5 * (Dice + CE), CE without ignore_index (:127,:178-180) ----
         probs, st = Bf("probs_l", (B, C, H, W)), Bf("stats_l", (2,))
@@ -564,16 +544,8 @@ class USTMStep(UAMTStep):
     def __init__(self, model, ema_model, base_lr=0.01, max_iterations=60000, ema_decay=0.99, **kw):
         super().__init__(model, ema_model, base_lr=base_lr, max_iterations=max_iterations, **kw)
         self.ema_decay = float(ema_decay)
-        tparams = self.ex_t.params
-        n = sum(p.numel() for p in tparams)
-        self.tflat = torch.empty(n, dtype=torch.float32, device=self.dev)
-        off = 0
-        for p in tparams:
-            self.tflat[off:off + p.numel()].copy_(p.data.reshape(-1))
-            p.data = self.tflat[off:off + p.numel()].view_as(p)
-            off += p.numel()
+        self.tflat, _ = _flatten(self.ex_t.params, self.dev)
         self.ramp_dev = torch.zeros(3, dtype=torch.float32, device=self.dev)     # {threshold, weight, 1 - EMA alpha}
-        self._graphs = {}
 
     def _ramps(self):
         import math
@@ -583,88 +555,38 @@ class USTMStep(UAMTStep):
         self.ramp_dev.copy_(torch.tensor([thr, cw, 1.0 - alpha], dtype=torch.float32))
         return thr, cw, alpha
 
-    def _finish(self, g, alpha):
-        """SGD on the student, then the EMA teacher update (:163).  alpha=None (captured): the factor is read from ramp_dev"""
+    def _finish(self, g, captured):
+        """SGD on the student, then the EMA teacher update (:163): eager with the host alpha, captured with the factor from ramp_dev"""
         self._opt(g)
         n = min(self.tflat.numel(), self.flat.numel())
-        if alpha is None:
+        if captured:
             self.tflat[:n].lerp_(self.flat[:n], self.ramp_dev[2])        # t + (1 - alpha) * (s - t)
         else:
-            call("wsl_ema_update", self.tflat, self.flat, n, float(alpha))
+            call("wsl_ema_update", self.tflat, self.flat, n, float(self._alpha))
 
     def __call__(self, image, label, noises=None, rot_times=None):
         self.model.train()
         self.ema_model.train()
         assert image.shape[2] == image.shape[3], "rot90 consistency needs square inputs"
-        k = random.randrange(0, 4) if rot_times is None else int(rot_times)
-        self.rot_times = k
-        thr, cw, alpha = self._ramps()
-        if not self.graph_enabled:
-            loss, g = self._body(image, label, noises, k)
-            if self.world_size > 1:
-                ddp.allreduce_flat(g[: self.n_trained], self.pg)
-            self._finish(g, alpha)
-        else:
-            assert noises is None, "graph mode draws the teacher noise on the device"
-            if self._static is None:
-                self._static = (torch.empty_like(image), torch.empty_like(label))
-            si, sl = self._static
-            assert si.shape == image.shape, "graph mode needs a fixed batch shape"
-            si.copy_(image, non_blocking=True)
-            sl.copy_(label, non_blocking=True)
-            if self._warm < 2:
-                c0 = _lib.COUNTERS["launch_calls"]
-                loss, g = self._body(si, sl, None, k)
-                if self.world_size > 1:
-                    ddp.allreduce_flat(g[: self.n_trained], self.pg)
-                self._finish(g, alpha)
-                self.launches_per_step = _lib.COUNTERS["launch_calls"] - c0
-                self._warm += 1
-            else:
-                if k not in self._graphs:
-                    torch.cuda.synchronize()
-                    g1, g2 = torch.cuda.CUDAGraph(), None
-                    with torch.cuda.graph(g1):
-                        gloss, gg = self._body(si, sl, None, k)
-                        if self.world_size == 1:
-                            self._finish(gg, None)
-                    if self.world_size > 1:
-                        g2 = torch.cuda.CUDAGraph()
-                        with torch.cuda.graph(g2):
-                            self._finish(gg, None)
-                    self._graphs[k] = (g1, g2, gloss, gg, dict(self.parts))
-                    self.comm_mode = "two graphs per rot90 count, host-issued all-reduce"
-                g1, g2, gloss, gg, self.parts = self._graphs[k]
-                g1.replay()
-                if g2 is not None:
-                    ddp.allreduce_flat(gg[: self.n_trained], self.pg)
-                    g2.replay()
-                loss = gloss.clone()
+        self.rot_times = random.randrange(0, 4) if rot_times is None else int(rot_times)
+        thr, cw, self._alpha = self._ramps()
+        assert noises is None or not self.graph_enabled, "graph mode draws the teacher noise on the device"
+        loss = self._run((image, label), key=self.rot_times, noises=noises)
         self.parts = dict(self.parts, weight=cw, threshold=thr)
-        lr_ = self.base_lr * (1.0 - self.iter_num / self.max_iterations) ** 0.9
-        self.lr_dev.fill_(lr_)
-        self.iter_num += 1
         return loss
 
-    def _body(self, image, label, noises, k):
-        ex, ex_t, dev = self.ex, self.ex_t, self.dev
+    def _fwd_bwd(self, image, label, noises=None):
+        ex, dev = self.ex, self.dev
         B, _, H, W = image.shape
-        C, T = 4, self.T
+        C, T, k = 4, self.T, self.rot_times
         self.seed_dev.add_(1)
         masks, ck = getattr(self.model, "dropout_masks", None), getattr(self.model, "channel_keep", None)
-        tmasks, tck = getattr(self.ema_model, "dropout_masks", None), getattr(self.ema_model, "channel_keep", None)
         outs, slot = ex.forward(image.contiguous(), True, True, masks, ck)
         out = outs[0]
         Bf = lambda name, shape, dt=torch.float32: ex.buf("ustm", name, shape, dt)
         rimg = Bf("rimg", (B, 1, H, W))
         call("wsl_rot90", image.contiguous(), B, H, k, 0, rimg)
-        ema_out = ex_t.forward(self._noisy(rimg, 1, 0, None if noises is None else noises[0]), True, False, tmasks, tck)[0][0]
-        mc = Bf("mc", (T * B, C, H, W))
-        for i in range(T // 2):
-            tm2 = None if tmasks is None else {kk: v.repeat(2, 1, 1, 1) for kk, v in tmasks.items()}
-            tck2 = None if tck is None else [c.repeat(2, 1) for c in tck]
-            lg = ex_t.forward(self._noisy(rimg, 2, 1 + i, None if noises is None else noises[1 + i]), True, False, tm2, tck2)[0][0]
-            mc[2 * B * i: 2 * B * (i + 1)].copy_(lg)
+        ema_out, mc = self._teacher(rimg, noises)
         # pCE (ignore_index 4)
         probs, st = Bf("probs", (B, C, H, W)), Bf("stats", (2,))
         call("wsl_softmax_pce_fwd", out, label, probs, B, C, H, W, 4, st, workspace("pce", dev))
@@ -707,7 +629,10 @@ class S2LStep(TrainStep):
         self.ctrl = torch.tensor([self.thr_conf, 0.0], dtype=torch.float32, device=self.dev)    # {thr_conf, w_u}
         self._w_u = 0.0
         self._weight = None
-        self._wstatic = None
+
+    def _fwd_bwd(self, image, label, weight):
+        self._weight = weight.contiguous()          # read by _head
+        return super()._fwd_bwd(image, label)
 
     def _head(self, logits_list, image, label, slot):
         ex = self.ex
@@ -724,22 +649,16 @@ class S2LStep(TrainStep):
 
     def __call__(self, image, scribble, weight):
         """image fp32 [N,1,H,W], scribble uint8 [N,H,W] (4 = unlabelled), weight fp32 [N,H,W,4] (S2LLoader's batch).  Returns the
-        loss (0-dim device tensor): NaN after thr_iter when no unlabelled pixel clears thr_conf, as the reference."""
+        loss (0-dim device tensor): NaN after thr_iter when no unlabelled pixel clears thr_conf, as the reference.
+        Graph mode: ``input_buffers(0/1)`` are (image, scribble, weight) triples."""
+        assert image.is_cuda and scribble.is_cuda and scribble.dtype == torch.uint8
         assert weight.is_cuda and weight.dtype == torch.float32 and tuple(weight.shape) == (image.shape[0],) + tuple(image.shape[2:]) + (4,)
         w_u = 0.5 if self.iter_num >= self.thr_iter else 0.0
         if w_u != self._w_u:
             self.ctrl[1].fill_(w_u)
             self._w_u = w_u
-        if self.graph_enabled:
-            if self._wstatic is None:
-                self._wstatic = torch.empty_like(weight)
-            assert self._wstatic.shape == weight.shape, "graph mode needs a fixed batch shape"
-            if self._wstatic.data_ptr() != weight.data_ptr():
-                self._wstatic.copy_(weight, non_blocking=True)
-            self._weight = self._wstatic
-        else:
-            self._weight = weight.contiguous()
-        return super().__call__(image, scribble)
+        self.model.train()
+        return self._run((image, scribble, weight))
 
     @torch.no_grad()
     def refresh(self, store, alpha=0.2, chunk=64, size=256, masks=None):
