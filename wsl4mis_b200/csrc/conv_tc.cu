@@ -21,6 +21,7 @@
 #include <mutex>
 #include <unordered_map>
 #include <string>
+#include <type_traits>
 #include <string.h>
 #include <stdlib.h>
 
@@ -153,7 +154,7 @@ struct ConvSmem {
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-template <int KBLK, int NT, int STAGES>
+template <int KBLK, int NT, int STAGES, int DT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0,
                                                                  const __grid_constant__ CUtensorMap map_a1,
                                                                  const __grid_constant__ CUtensorMap map_b, const ConvTcParams p) {
@@ -220,8 +221,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < KBLK / 16; ++k)   // 16 elements (32 bytes) along K inside the swizzle span
-      Wgmma<NT>::template mma<0, 0>(acc, gmma_desc<SW>(a_addr + 32 * k, 16, 8 * SW), gmma_desc<SW>(b_addr + 32 * k, 16, 8 * SW),
-                                    (it > 0 || k > 0) ? 1u : 0u, p.dt);
+      Wgmma<NT>::template mma<0, 0, DT>(acc, gmma_desc<SW>(a_addr + 32 * k, 16, 8 * SW), gmma_desc<SW>(b_addr + 32 * k, 16, 8 * SW),
+                                        (it > 0 || k > 0) ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
     release_stage(&empty_bar[s]);
@@ -240,7 +241,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
       float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
       if (p.out_scale) { v0 *= sc; v1 *= sc; }
       if (p.bias) { v0 += p.bias[c]; v1 += p.bias[c + 1]; }
-      store_pair(p.out, p.out_mode, p.dt, p.CoutStore, p.H, p.W, n, gy, gx, c, v0, v1);
+      store_pair(p.out, p.out_mode, DT, p.CoutStore, p.H, p.W, n, gy, gx, c, v0, v1);
     }
   }
 }
@@ -318,30 +319,39 @@ int get_map(const void* ptr, int rank, const long long* dims, const int* box, in
   return 0;
 }
 
-template <int KBLK, int NT, int STAGES>
+// Calls f(std::integral_constant<int, DT>) with the 16-bit operand type dt (0 bf16, 2 fp16) as a compile-time constant.
+template <class F>
+int with_dt(int dt, F&& f) {
+  return dt == 2 ? f(std::integral_constant<int, 2>{}) : f(std::integral_constant<int, 0>{});
+}
+
+template <int KBLK, int NT, int STAGES, int DT>
 int launch_conv(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvTcParams& p, cudaStream_t stream) {
   using S = ConvSmem<KBLK, NT, STAGES>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<KBLK, NT, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<KBLK, NT, STAGES, DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
     if (e != cudaSuccess) { wsl_set_error("conv_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return -5; }
     attr = true;
   }
   dim3 grid(p.N * p.tiles_x * p.tiles_y, p.CoutP / NT);
-  conv_tc_kernel<KBLK, NT, STAGES><<<grid, NUM_THREADS, S::TOTAL, stream>>>(a0, a1, b, p);
+  conv_tc_kernel<KBLK, NT, STAGES, DT><<<grid, NUM_THREADS, S::TOTAL, stream>>>(a0, a1, b, p);
   return wsl_check_launch("conv_tc");
 }
 
 template <int KBLK>
 int dispatch_nt(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvTcParams& p, int nt, cudaStream_t stream) {
-  switch (nt) {
-    case 16:  return launch_conv<KBLK, 16, 6>(a0, a1, b, p, stream);
-    case 32:  return launch_conv<KBLK, 32, 6>(a0, a1, b, p, stream);
-    case 64:  return launch_conv<KBLK, 64, 6>(a0, a1, b, p, stream);
-    case 128: return launch_conv<KBLK, 128, 5>(a0, a1, b, p, stream);
-  }
-  wsl_set_error("conv_tc: unsupported N tile %d", nt);
-  return -1;
+  return with_dt(p.dt, [&](auto dt) {
+    constexpr int DT = decltype(dt)::value;
+    switch (nt) {
+      case 16:  return launch_conv<KBLK, 16, 6, DT>(a0, a1, b, p, stream);
+      case 32:  return launch_conv<KBLK, 32, 6, DT>(a0, a1, b, p, stream);
+      case 64:  return launch_conv<KBLK, 64, 6, DT>(a0, a1, b, p, stream);
+      case 128: return launch_conv<KBLK, 128, 5, DT>(a0, a1, b, p, stream);
+    }
+    wsl_set_error("conv_tc: unsupported N tile %d", nt);
+    return -1;
+  });
 }
 
 
@@ -415,7 +425,7 @@ __device__ __forceinline__ void write_stat_partials(float (&rs)[NT / 4], float (
   }
 }
 
-template <int KS, int KBLK, int NT, int MT, int STAGES>
+template <int KS, int KBLK, int NT, int MT, int STAGES, int DT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc2_kernel(const __grid_constant__ CUtensorMap map_a0,
                                                                   const __grid_constant__ CUtensorMap map_a1,
                                                                   const __grid_constant__ CUtensorMap map_b, const ConvV2Params p,
@@ -502,16 +512,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc2_kernel(const __grid_c
           const int dy = tap / KS, dx = tap % KS;
 #pragma unroll
           for (int k = 0; k < KBLK / 16; ++k)
-            Wgmma<NT>::template mma<0, 0>(acc[j],
-                                          gmma_desc<SW>(a_base + (uint32_t)(((16 * j + dy) * Cfg::HW_ + dx) * Cfg::ROWB + 32 * k), 16, Cfg::HW_ * Cfg::ROWB),
-                                          gmma_desc<SW>(w_base + (uint32_t)(tap * nkb * Cfg::W_SUB + 32 * k), 16, 8 * SW),
-                                          (kb > 0 || tap > 0 || k > 0) ? 1u : 0u, p.dt);
+            Wgmma<NT>::template mma<0, 0, DT>(acc[j],
+                                              gmma_desc<SW>(a_base + (uint32_t)(((16 * j + dy) * Cfg::HW_ + dx) * Cfg::ROWB + 32 * k), 16, Cfg::HW_ * Cfg::ROWB),
+                                              gmma_desc<SW>(w_base + (uint32_t)(tap * nkb * Cfg::W_SUB + 32 * k), 16, 8 * SW),
+                                              (kb > 0 || tap > 0 || k > 0) ? 1u : 0u);
         }
       }
       wgmma_commit();
-      wgmma_wait<0>();
-      release_stage(&a_empty[s]);
+      wgmma_wait<1>();                     // the previous k-block's group has retired: its stage can be refilled
+      if (kb > 0) release_stage(&a_empty[(it + STAGES - 1) % STAGES]);
     }
+    wgmma_wait<0>();
+    release_stage(&a_empty[(it + STAGES - 1) % STAGES]);
 #pragma unroll
     for (int j = 0; j < MT; ++j) {
       wgmma_fence_regs(acc[j]);
@@ -526,12 +538,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc2_kernel(const __grid_c
           if (p.bias) { v0 += p.bias[n0 + c]; v1 += p.bias[n0 + c + 1]; }
           if (p.out_mode == 0 && p.stat_partials) {   // BatchNorm statistics of the values exactly as stored
             float2 r;
-            if (p.dt == 2) r = __half22float2(__floats2half2_rn(v0, v1));
+            if (DT == 2) r = __half22float2(__floats2half2_rn(v0, v1));
             else r = __bfloat1622float2(__floats2bfloat162_rn(v0, v1));
             rs[2 * jj] += r.x;     rq[2 * jj] += r.x * r.x;
             rs[2 * jj + 1] += r.y; rq[2 * jj + 1] += r.y * r.y;
           }
-          store_pair(p.out, p.out_mode == 0 ? 0 : 1, p.dt, p.CoutStore, p.H, p.W, n, gy, gx, n0 + c, v0, v1);
+          store_pair(p.out, p.out_mode == 0 ? 0 : 1, DT, p.CoutStore, p.H, p.W, n, gy, gx, n0 + c, v0, v1);
         }
       }
     }
@@ -580,7 +592,7 @@ struct WgradSmem {
   static constexpr int TOTAL = STAGES * STAGE_BYTES + SLACK + 1024 + 256;
 };
 
-template <int CWA, int NA, int CWB, int TG, int STAGES>
+template <int CWA, int NA, int CWB, int TG, int STAGES, int DT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy,
                                                                   const __grid_constant__ CUtensorMap map_x0,
                                                                   const __grid_constant__ CUtensorMap map_x1, const WgradTcParams p) {
@@ -660,9 +672,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const __grid_c
       for (int tl = 0; tl < TG; ++tl) {
 #pragma unroll
         for (int k = 0; k < TILE_M / 16; ++k)   // 16 pixels (rows) per MMA: advance both operands by 16 rows
-          Wgmma<CWB>::template mma<1, 1>(acc[tl], gmma_desc<SWA>(a_addr + (uint32_t)(k * 16 * SWA), S::A_BOX, 8 * SWA),
-                                         gmma_desc<SWB>(b_addr + (uint32_t)(tl * S::B_BOX + k * 16 * SWB), S::B_BOX, 8 * SWB),
-                                         (it > 0 || k > 0) ? 1u : 0u, p.dt);
+          Wgmma<CWB>::template mma<1, 1, DT>(acc[tl], gmma_desc<SWA>(a_addr + (uint32_t)(k * 16 * SWA), S::A_BOX, 8 * SWA),
+                                             gmma_desc<SWB>(b_addr + (uint32_t)(tl * S::B_BOX + k * 16 * SWB), S::B_BOX, 8 * SWB),
+                                             (it > 0 || k > 0) ? 1u : 0u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -707,7 +719,7 @@ struct Wgrad2Smem {
   static constexpr int TOTAL = STAGES * STAGE_BYTES + SLACK + 1024 + 256;
 };
 
-template <int CWA, int NA, int CWB, int STAGES>
+template <int CWA, int NA, int CWB, int STAGES, int DT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc2_kernel(const __grid_constant__ CUtensorMap map_dy,
                                                                    const __grid_constant__ CUtensorMap map_x0,
                                                                    const __grid_constant__ CUtensorMap map_x1, const WgradTcParams p) {
@@ -779,9 +791,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc2_kernel(const __grid_
 #pragma unroll
         for (int k = 0; k < 8; ++k)
           // k-step = 16 pixels = image rows 2k, 2k+1 of the chunk: A advances 16 rows, B advances 2 halo rows
-          Wgmma<CWB>::template mma<1, 1>(acc[tap], gmma_desc<SWA>(a_addr + (uint32_t)(k * 16 * SWA), S::A_BOX, 8 * SWA),
-                                         gmma_desc<SWB>(b_addr + (uint32_t)((dy * 10 + dx) * S::ROWB + k * 2 * 10 * S::ROWB), S::B_HALO, 10 * S::ROWB),
-                                         (it > 0 || k > 0) ? 1u : 0u, p.dt);
+          Wgmma<CWB>::template mma<1, 1, DT>(acc[tap], gmma_desc<SWA>(a_addr + (uint32_t)(k * 16 * SWA), S::A_BOX, 8 * SWA),
+                                             gmma_desc<SWB>(b_addr + (uint32_t)((dy * 10 + dx) * S::ROWB + k * 2 * 10 * S::ROWB), S::B_HALO, 10 * S::ROWB),
+                                             (it > 0 || k > 0) ? 1u : 0u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -806,7 +818,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc2_kernel(const __grid_
   }
 }
 
-template <int CWA, int NA, int CWB>
+template <int CWA, int NA, int CWB, int DT>
 int launch_wgrad2(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorMap& mx1, const WgradTcParams& p, int m_tiles,
                   cudaStream_t stream) {
   constexpr int per_stage = NA * TILE_M * CWA * 2 + 12 * 1024;
@@ -814,7 +826,7 @@ int launch_wgrad2(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensor
   using S = Wgrad2Smem<CWA, NA, CWB, STAGES>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc2_kernel<CWA, NA, CWB, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tc2_kernel<CWA, NA, CWB, STAGES, DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
     if (e != cudaSuccess) { wsl_set_error("wgrad_tc2: cudaFuncSetAttribute(%d bytes): %s", S::TOTAL, cudaGetErrorString(e)); return -5; }
     attr = true;
   }
@@ -823,7 +835,7 @@ int launch_wgrad2(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensor
   if (splits > p.nchunks) splits = p.nchunks;
   if (splits < 1) splits = 1;
   dim3 grid(splits, gy);
-  wgrad_tc2_kernel<CWA, NA, CWB, STAGES><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
+  wgrad_tc2_kernel<CWA, NA, CWB, STAGES, DT><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
   return wsl_check_launch("wgrad_tc2");
 }
 
@@ -862,7 +874,7 @@ struct Wgrad3Params {
   float* partials;            // optional [gridDim.y][gridDim.x][3*NTILE][128]: per-CTA partial tiles for the fixed-order finalize
 };
 
-template <int CWB, int NTILE, int STAGES>
+template <int CWB, int NTILE, int STAGES, int DT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc3_kernel(const __grid_constant__ CUtensorMap map_dy,
                                                                    const __grid_constant__ CUtensorMap map_x0,
                                                                    const __grid_constant__ CUtensorMap map_x1, const Wgrad3Params p) {
@@ -927,8 +939,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc3_kernel(const __grid_
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < 8; ++k)      // k-step = 16 pixels = chunk rows 2k, 2k+1
-        Wgmma<NG>::template mma<1, 1>(acc, gmma_desc<SWX>(a_addr + (uint32_t)(k * 2 * 10 * S::ROWB), S::ROWB, 10 * S::ROWB),
-                                      gmma_desc<SWN>(b_addr + (uint32_t)(k * 16 * SWN), 8 * SWN, 8 * SWN), (it > 0 || k > 0) ? 1u : 0u, p.dt);
+        Wgmma<NG>::template mma<1, 1, DT>(acc, gmma_desc<SWX>(a_addr + (uint32_t)(k * 2 * 10 * S::ROWB), S::ROWB, 10 * S::ROWB),
+                                          gmma_desc<SWN>(b_addr + (uint32_t)(k * 16 * SWN), 8 * SWN, 8 * SWN), (it > 0 || k > 0) ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<0>();
     }
@@ -988,7 +1000,7 @@ __global__ void __launch_bounds__(256) wgrad3_finalize_kernel(const float* __res
   dw[((size_t)co * CinTot + ci_global + ci) * 9 + dy * 3 + g] += acc;
 }
 
-template <int CWB, int NTILE>
+template <int CWB, int NTILE, int DT>
 int launch_wgrad3(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorMap& mx1, Wgrad3Params p, int n_tiles,
                   float* partial_ws, long long partial_floats, cudaStream_t stream) {
   constexpr int per_stage = TILE_M * NTILE * 2 + 12 * 1024;
@@ -996,13 +1008,13 @@ int launch_wgrad3(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensor
   using S = Wgrad3Smem<CWB, NTILE, STAGES>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc3_kernel<CWB, NTILE, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tc3_kernel<CWB, NTILE, STAGES, DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
     if (e != cudaSuccess) { wsl_set_error("wgrad_tc3: cudaFuncSetAttribute(%d bytes): %s", S::TOTAL, cudaGetErrorString(e)); return -5; }
     attr = true;
   }
   const int gy = n_tiles * (p.k_tiles0 + p.k_tiles1);
   int per_sm = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wgrad_tc3_kernel<CWB, NTILE, STAGES>, NUM_THREADS, S::TOTAL);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wgrad_tc3_kernel<CWB, NTILE, STAGES, DT>, NUM_THREADS, S::TOTAL);
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 2) per_sm = 2;
   int splits = (wsl_num_sms() * per_sm + gy - 1) / gy;
@@ -1011,7 +1023,7 @@ int launch_wgrad3(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensor
   dim3 grid(splits, gy);
   const long long need = (long long)splits * gy * 3 * NTILE * 128;
   p.partials = (partial_ws != nullptr && need <= partial_floats) ? partial_ws : nullptr;     // too small a workspace: atomics
-  wgrad_tc3_kernel<CWB, NTILE, STAGES><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
+  wgrad_tc3_kernel<CWB, NTILE, STAGES, DT><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
   int rc = wsl_check_launch("wgrad_tc3");
   if (rc || p.partials == nullptr) return rc;
   wgrad3_finalize_kernel<<<dim3((3 * NTILE * 128 + 255) / 256, gy), 256, 0, stream>>>(p.partials, splits, NTILE, CWB, 1, p.k_tiles0,
@@ -1051,7 +1063,7 @@ __global__ void __launch_bounds__(256) wgrad1_finalize_kernel(const float* __res
 static thread_local float* g_wgrad1_ws = nullptr;        // set by the entry point for the launch helpers below
 static thread_local long long g_wgrad1_ws_floats = 0;
 
-template <int CWA, int NA, int CWB, int TG>
+template <int CWA, int NA, int CWB, int TG, int DT>
 int launch_wgrad(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorMap& mx1, WgradTcParams p, int m_tiles,
                  cudaStream_t stream) {
   constexpr int per_stage = NA * TILE_M * CWA * 2 + TG * TILE_M * CWB * 2;
@@ -1059,7 +1071,7 @@ int launch_wgrad(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorM
   using S = WgradSmem<CWA, NA, CWB, TG, STAGES>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<CWA, NA, CWB, TG, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<CWA, NA, CWB, TG, STAGES, DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
     if (e != cudaSuccess) { wsl_set_error("wgrad_tc: cudaFuncSetAttribute(%d bytes): %s", S::TOTAL, cudaGetErrorString(e)); return -5; }
     attr = true;
   }
@@ -1070,7 +1082,7 @@ int launch_wgrad(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorM
   dim3 grid(splits, gy);
   const long long need = (long long)splits * gy * TG * CWB * 128;
   p.partials = (g_wgrad1_ws != nullptr && need <= g_wgrad1_ws_floats) ? g_wgrad1_ws : nullptr;
-  wgrad_tc_kernel<CWA, NA, CWB, TG, STAGES><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
+  wgrad_tc_kernel<CWA, NA, CWB, TG, STAGES, DT><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
   int rc = wsl_check_launch("wgrad_tc");
   if (rc || p.partials == nullptr) return rc;
   wgrad1_finalize_kernel<<<dim3((TG * CWB * 128 + 255) / 256, gy), 256, 0, stream>>>(p.partials, splits, TG, CWB, p.tap_groups, p.n_tiles0,
@@ -1081,8 +1093,11 @@ int launch_wgrad(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorM
 
 template <int CWA, int NA, int CWB>
 int wgrad_dispatch_tg(const CUtensorMap& a, const CUtensorMap& b0, const CUtensorMap& b1, const WgradTcParams& p, int m_tiles, cudaStream_t st) {
-  if (p.ks == 3) return launch_wgrad<CWA, NA, CWB, 3>(a, b0, b1, p, m_tiles, st);
-  return launch_wgrad<CWA, NA, CWB, 1>(a, b0, b1, p, m_tiles, st);
+  return with_dt(p.dt, [&](auto dt) {
+    constexpr int DT = decltype(dt)::value;
+    if (p.ks == 3) return launch_wgrad<CWA, NA, CWB, 3, DT>(a, b0, b1, p, m_tiles, st);
+    return launch_wgrad<CWA, NA, CWB, 1, DT>(a, b0, b1, p, m_tiles, st);
+  });
 }
 template <int CWA, int NA>
 int wgrad_dispatch_b(int cwb, const CUtensorMap& a, const CUtensorMap& b0, const CUtensorMap& b1, const WgradTcParams& p, int m_tiles, cudaStream_t st) {
@@ -1172,7 +1187,7 @@ __global__ void __launch_bounds__(256) channel_sum_kernel(const T* __restrict__ 
 
 static int g_conv2_last_rows = 0;   // gridDim.x of the most recent conv_tc2 launch (rows of stat_partials)
 
-template <int KS, int KBLK, int NT, int MT>
+template <int KS, int KBLK, int NT, int MT, int DT>
 int launch_conv2(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, cudaStream_t stream) {
   using Cfg = ConvV2Cfg<KS, KBLK, NT, MT>;
   constexpr int STAGES = (Cfg::A_STAGE <= 8 * 1024) ? 4 : (Cfg::A_STAGE <= 13 * 1024) ? 3 : 2;
@@ -1183,33 +1198,36 @@ int launch_conv2(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap
   if (smem > 227 * 1024) { wsl_set_error("conv_tc2: %d bytes of shared memory needed", smem); return -6; }
   static int attr_bytes = 0;
   if (smem > attr_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<KS, KBLK, NT, MT, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<KS, KBLK, NT, MT, STAGES, DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { wsl_set_error("conv_tc2: cudaFuncSetAttribute(%d): %s", smem, cudaGetErrorString(e)); return -5; }
     attr_bytes = smem;
   }
   const int n_tiles = p.CoutP / NT;
   int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_tc2_kernel<KS, KBLK, NT, MT, STAGES>, NUM_THREADS, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_tc2_kernel<KS, KBLK, NT, MT, STAGES, DT>, NUM_THREADS, smem);
   if (occ < 1) occ = 1;
   int gx = (wsl_num_sms() * occ) / n_tiles;
   if (gx < 1) gx = 1;
   if (gx > p.ntiles) gx = p.ntiles;
   dim3 grid(gx, n_tiles);
   g_conv2_last_rows = gx;
-  conv_tc2_kernel<KS, KBLK, NT, MT, STAGES><<<grid, NUM_THREADS, smem, stream>>>(a0, a1, b, p, w_bytes);
+  conv_tc2_kernel<KS, KBLK, NT, MT, STAGES, DT><<<grid, NUM_THREADS, smem, stream>>>(a0, a1, b, p, w_bytes);
   return wsl_check_launch("conv_tc2");
 }
 
 template <int KS, int KBLK, int MT>
 int conv2_dispatch_nt(int nt, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, cudaStream_t st) {
-  switch (nt) {
-    case 16:  return launch_conv2<KS, KBLK, 16, MT>(a0, a1, b, p, st);
-    case 32:  return launch_conv2<KS, KBLK, 32, MT>(a0, a1, b, p, st);
-    case 64:  if constexpr (MT <= 2) return launch_conv2<KS, KBLK, 64, MT>(a0, a1, b, p, st); else break;
-    case 128: if constexpr (MT == 1) return launch_conv2<KS, KBLK, 128, MT>(a0, a1, b, p, st); else break;
-  }
-  wsl_set_error("conv_tc2: unsupported N tile %d", nt);
-  return -1;
+  return with_dt(p.dt, [&](auto dt) {
+    constexpr int DT = decltype(dt)::value;
+    switch (nt) {
+      case 16:  return launch_conv2<KS, KBLK, 16, MT, DT>(a0, a1, b, p, st);
+      case 32:  return launch_conv2<KS, KBLK, 32, MT, DT>(a0, a1, b, p, st);
+      case 64:  if constexpr (MT <= 2) return launch_conv2<KS, KBLK, 64, MT, DT>(a0, a1, b, p, st); else break;
+      case 128: if constexpr (MT == 1) return launch_conv2<KS, KBLK, 128, MT, DT>(a0, a1, b, p, st); else break;
+    }
+    wsl_set_error("conv_tc2: unsupported N tile %d", nt);
+    return -1;
+  });
 }
 
 // ================================================================================================
@@ -1222,16 +1240,37 @@ int conv2_dispatch_nt(int nt, const CUtensorMap& a0, const CUtensorMap& a1, cons
 //     out[r][c] = E_r[c][dy=0] + E_{r+1}[c][dy=1] + E_{r+2}[c][dy=2]
 // summed in registers by the thread that owns pixel c (a rolling pair of partial rows): no cross-thread traffic.
 //   warp 8: TMA producer (one [KBW ch x 130 px] box per input row and channel block; OOB zero fill = padding)
-//   warpgroup h: pixels 64h .. 64h+63 of the strip (MMA issue + epilogue).
+//   warpgroup h: pixels 64h .. 64h+63 of the strip (MMA issue + epilogue).  The MMAs of input row i + 1 are issued before
+//   the output row that row i completes is stored, so the tensor core works through the stores.
 // Work item = (image, 128-pixel column strip, segment of RS output rows); persistent CTAs walk the items.
 // ================================================================================================
 constexpr int ROW_PX = 128;
 // bytes of one input-row buffer: 130 halo pixels x KBW channels, padded to a multiple of the 8-row swizzle atom
 __host__ __device__ constexpr int row_abytes(int kbw) { return ((130 * kbw * 2 + 255) / 256) * 256; }
 
-template <int NT, int KBW>
+// The MMAs of one input row (KB channel blocks x KBW/16 k-steps x 3 pixel shifts) into acc as one commit group.  The first
+// has scale-d = 0, so acc needs no zero fill: no other instruction writes accumulator registers while a group is in flight.
+template <int NT, int KBW, int KB, int DT>
+__device__ __forceinline__ void row_mma(float (&acc)[3 * NT / 2], uint32_t a_row, uint32_t w_u) {
+  constexpr int NG = 3 * NT, SWB = KBW * 2, ROW_ABYTES = row_abytes(KBW);
+  wgmma_fence();
+#pragma unroll
+  for (int kb = 0; kb < KB; ++kb) {
+#pragma unroll
+    for (int ks = 0; ks < KBW / 16; ++ks) {
+#pragma unroll
+      for (int dx = 0; dx < 3; ++dx)
+        Wgmma<NG>::template mma<0, 0, DT>(acc, gmma_desc<SWB>(a_row + (uint32_t)(kb * ROW_ABYTES + dx * SWB + 32 * ks), 16, 8 * SWB),
+                                          gmma_desc<SWB>(w_u + (uint32_t)((kb * 3 + dx) * NG * SWB + 32 * ks), 16, 8 * SWB),
+                                          (kb > 0 || ks > 0 || dx > 0) ? 1u : 0u);
+    }
+  }
+  wgmma_commit();
+}
+
+template <int NT, int KBW, int KB, int DT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
-                                                                  const __grid_constant__ CUtensorMap map_b, const ConvV2Params p, const int KB,
+                                                                  const __grid_constant__ CUtensorMap map_b, const ConvV2Params p,
                                                                   const int RS, const int w_bytes, const int STAGES) {
   constexpr int NG = 3 * NT;                              // accumulator columns of one input row (three filter rows)
   constexpr int SWB = KBW * 2, ROW_ABYTES = row_abytes(KBW);   // channel block = swizzle span: 32 B (16 ch) or 64 B (32 ch)
@@ -1312,8 +1351,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_c
 #pragma unroll
   for (int k = 0; k < NT / 4; ++k) ls[k] = lq[k] = 0.f;
   mbar_wait(w_bar, 0);
-  int s = 0;
+  int s = 0, rel = 0;                   // next stage to consume / stage of the row whose MMA group is in flight
   uint32_t sph = 0;
+  // One accumulator, one MMA group in flight: row i's group is folded into the partial rows as soon as it retires, then the
+  // group of the next row (of this item or the next one) is issued and runs while row i - 2 is rounded and stored.  A second
+  // accumulator would keep 3*NT/2 more floats live and spill under the 168-register limit of a 384-thread CTA.
+  float acc[NG / 2];
+  if (my_items > 0) {
+    mbar_wait(&a_full[s], sph);
+    row_mma<NT, KBW, KB, DT>(acc, a_u + (uint32_t)(s * KB * ROW_ABYTES), w_u);
+    if (++s == STAGES) { s = 0; sph ^= 1u; }
+  }
   for (int it = 0; it < my_items; ++it) {
     const int item = blockIdx.x + it * gridDim.x;
     const int seg = item % segs, t1 = item / segs, strip = t1 % strips, n = t1 / strips;
@@ -1322,29 +1370,28 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_c
 #pragma unroll
     for (int e = 0; e < NT / 2; ++e) pa[e] = pb[e] = 0.f;
     for (int i = 0; i < rows_in; ++i) {
-      float acc[NG / 2];
-#pragma unroll
-      for (int e = 0; e < NG / 2; ++e) acc[e] = 0.f;
-      mbar_wait(&a_full[s], sph);
-      wgmma_fence();
-      for (int kb = 0; kb < KB; ++kb) {
-        const uint32_t a_lo = a_u + (uint32_t)((s * KB + kb) * ROW_ABYTES);
-        const uint32_t w_lo = w_u + (uint32_t)(kb * 3 * NG * SWB);
-#pragma unroll
-        for (int ks = 0; ks < KBW / 16; ++ks) {
-#pragma unroll
-          for (int dx = 0; dx < 3; ++dx)
-            Wgmma<NG>::template mma<0, 0>(acc, gmma_desc<SWB>(a_lo + (uint32_t)(dx * SWB + 32 * ks), 16, 8 * SWB),
-                                          gmma_desc<SWB>(w_lo + (uint32_t)(dx * NG * SWB + 32 * ks), 16, 8 * SWB),
-                                          (kb > 0 || ks > 0 || dx > 0) ? 1u : 0u, p.dt);
-        }
-      }
-      wgmma_commit();
       wgmma_wait<0>();
-      release_stage(&a_empty[s]);
-      if (++s == STAGES) { s = 0; sph ^= 1u; }
+      release_stage(&a_empty[rel]);
+      if (++rel == STAGES) rel = 0;
       wgmma_fence_regs(acc);
       // column 8*j + frag_col + b of E: filter row j / (NT/8), output channel 8*(j % (NT/8)) + frag_col + b
+      float o[NT / 2];                  // output row i - 2 (i >= 2), before rounding to the 16-bit type
+#pragma unroll
+      for (int ii = 0; ii < 2; ++ii)
+#pragma unroll
+        for (int jj = 0; jj < NT / 8; ++jj)
+#pragma unroll
+          for (int b = 0; b < 2; ++b) {
+            const int e = 4 * jj + 2 * ii + b;
+            o[e] = (pa[e] + acc[4 * (2 * NT / 8 + jj) + 2 * ii + b]) + s_bias[8 * jj + frag_col(t) + b];
+            pa[e] = pb[e] + acc[4 * (NT / 8 + jj) + 2 * ii + b];   // output row i - 1: + filter row 1
+            pb[e] = acc[4 * jj + 2 * ii + b];                       // output row i: filter row 0
+          }
+      if (i + 1 < rows_in || it + 1 < my_items) {
+        mbar_wait(&a_full[s], sph);
+        row_mma<NT, KBW, KB, DT>(acc, a_u + (uint32_t)(s * KB * ROW_ABYTES), w_u);
+        if (++s == STAGES) { s = 0; sph ^= 1u; }
+      }
       if (i >= 2) {                                   // output row i - 2 is complete
         const int gy = y0 + i - 2;
 #pragma unroll
@@ -1353,36 +1400,25 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_c
 #pragma unroll
           for (int jj = 0; jj < NT / 8; ++jj) {
             const int c = 8 * jj + frag_col(t), e = 4 * jj + 2 * ii;
-            const float v0 = (pa[e] + acc[4 * (2 * NT / 8 + jj) + 2 * ii]) + s_bias[c];
-            const float v1 = (pa[e + 1] + acc[4 * (2 * NT / 8 + jj) + 2 * ii + 1]) + s_bias[c + 1];
+            const float v0 = o[e], v1 = o[e + 1];
             if (p.out_mode == 0 && p.stat_partials) {   // statistics of the values exactly as stored (rounded to the 16-bit type)
               float2 r;
-              if (p.dt == 2) r = __half22float2(__floats2half2_rn(v0, v1));
+              if (DT == 2) r = __half22float2(__floats2half2_rn(v0, v1));
               else r = __bfloat1622float2(__floats2bfloat162_rn(v0, v1));
               ls[2 * jj] += r.x;     lq[2 * jj] = fmaf(r.x, r.x, lq[2 * jj]);
               ls[2 * jj + 1] += r.y; lq[2 * jj + 1] = fmaf(r.y, r.y, lq[2 * jj + 1]);
             }
-            store_pair(p.out, p.out_mode == 0 ? 0 : 1, p.dt, p.CoutStore, p.H, p.W, n, gy, gx, c, v0, v1);
+            store_pair(p.out, p.out_mode == 0 ? 0 : 1, DT, p.CoutStore, p.H, p.W, n, gy, gx, c, v0, v1);
           }
         }
       }
-#pragma unroll
-      for (int ii = 0; ii < 2; ++ii)
-#pragma unroll
-        for (int jj = 0; jj < NT / 8; ++jj)
-#pragma unroll
-          for (int b = 0; b < 2; ++b) {
-            const int e = 4 * jj + 2 * ii + b;
-            pa[e] = pb[e] + acc[4 * (NT / 8 + jj) + 2 * ii + b];   // output row i - 1: + filter row 1
-            pb[e] = acc[4 * jj + 2 * ii + b];                       // output row i: filter row 0
-          }
     }
   }
   if (p.out_mode == 0 && p.stat_partials) write_stat_partials<NT>(ls, lq, p.stat_partials, p.CoutP, 0);
 }
 
-template <int NT, int KBW>
-int launch_conv_row(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, int KB, int RS,
+template <int NT, int KBW, int KB, int DT>
+int launch_conv_row(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, int RS,
                     cudaStream_t stream) {
   // Row buffers in flight: ~80 KB per SM cover the HBM latency.
   static const int st_env = [] { const char* e = getenv("WSL4MIS_ROW_STAGES"); return e ? atoi(e) : 0; }();
@@ -1392,19 +1428,33 @@ int launch_conv_row(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensor
   if (smem > 220 * 1024) { wsl_set_error("conv_row: %d bytes of shared memory needed", smem); return -6; }
   static int attr_bytes = 0;
   if (smem > attr_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(conv_row_kernel<NT, KBW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_row_kernel<NT, KBW, KB, DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { wsl_set_error("conv_row: cudaFuncSetAttribute(%d): %s", smem, cudaGetErrorString(e)); return -5; }
     attr_bytes = smem;
   }
   const int items = p.N * (p.W / ROW_PX) * (p.H / RS);
   int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_row_kernel<NT, KBW>, NUM_THREADS, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_row_kernel<NT, KBW, KB, DT>, NUM_THREADS, smem);
   if (occ < 1) occ = 1;
   int gx = wsl_num_sms() * occ;
   if (gx > items) gx = items;
   g_conv2_last_rows = gx;
-  conv_row_kernel<NT, KBW><<<gx, NUM_THREADS, smem, stream>>>(a0, a1, b, p, KB, RS, w_bytes, STAGES);
+  conv_row_kernel<NT, KBW, KB, DT><<<gx, NUM_THREADS, smem, stream>>>(a0, a1, b, p, RS, w_bytes, STAGES);
   return wsl_check_launch("conv_row");
+}
+
+// KB = (C0 + C1) / KBW channel blocks: 1-4 at KBW = 16, 1-2 at KBW = 32 (the caller keeps C0 + C1 <= 64)
+template <int NT, int KBW, int DT>
+int conv_row_dispatch_kb(int KB, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, int RS,
+                         cudaStream_t stream) {
+  switch (KB) {
+    case 1: return launch_conv_row<NT, KBW, 1, DT>(a0, a1, b, p, RS, stream);
+    case 2: return launch_conv_row<NT, KBW, 2, DT>(a0, a1, b, p, RS, stream);
+    case 3: if constexpr (KBW == 16) return launch_conv_row<NT, KBW, 3, DT>(a0, a1, b, p, RS, stream); else break;
+    case 4: if constexpr (KBW == 16) return launch_conv_row<NT, KBW, 4, DT>(a0, a1, b, p, RS, stream); else break;
+  }
+  wsl_set_error("conv_row: unsupported channel block count %d", KB);
+  return -1;
 }
 
 }  // namespace
@@ -1654,9 +1704,12 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
       p.tiles_x = 0; p.tiles_y = 0; p.ntiles = 0;
       p.out_mode = out_mode; p.dt = dtype; p.bias = bias; p.out = out;
       p.stat_partials = (out_mode == 0) ? stat_partials : nullptr;
-      const int rc = (CoutP == 16) ? launch_conv_row<16, 16>(a0, a1, b, p, KB, RS, stream)
-                     : (kbw == 32)   ? launch_conv_row<32, 32>(a0, a1, b, p, KB, RS, stream)
-                                     : launch_conv_row<32, 16>(a0, a1, b, p, KB, RS, stream);
+      const int rc = with_dt(dtype, [&](auto dt) {
+        constexpr int DT = decltype(dt)::value;
+        return (CoutP == 16) ? conv_row_dispatch_kb<16, 16, DT>(KB, a0, a1, b, p, RS, stream)
+               : (kbw == 32) ? conv_row_dispatch_kb<32, 32, DT>(KB, a0, a1, b, p, RS, stream)
+                             : conv_row_dispatch_kb<32, 16, DT>(KB, a0, a1, b, p, RS, stream);
+      });
       if (stat_rows_host) *stat_rows_host = g_conv2_last_rows;
       return rc;
     }
@@ -1758,10 +1811,13 @@ WSL_API int wsl_wgrad_tc2(const void* src0, int C0, const void* src1, int C1, co
   p.N = N; p.H = H; p.W = W; p.C0 = C0; p.C1 = C1; p.CoutP = CoutP; p.CoutReal = CoutReal; p.taps = 9; p.ks = 3;
   p.tiles_x = W / 8; p.tiles_y = H / 16; p.nchunks = N * p.tiles_x * p.tiles_y;
   p.n_tiles0 = C0 / cwb; p.n_tiles1 = C1 / cwb; p.tap_groups = 1; p.dt = dtype; p.scale_a = nullptr; p.scale_b = nullptr; p.dw = dw; p.partials = nullptr; p.dil = 1;
-  if (cwa == 64 && na == 2) return launch_wgrad2<64, 2, 16>(mdy, mx0, mx1, p, m_tiles, stream);
-  if (cwa == 64) return launch_wgrad2<64, 1, 16>(mdy, mx0, mx1, p, m_tiles, stream);
-  if (cwa == 32) return launch_wgrad2<32, 1, 16>(mdy, mx0, mx1, p, m_tiles, stream);
-  return launch_wgrad2<16, 1, 16>(mdy, mx0, mx1, p, m_tiles, stream);
+  return with_dt(dtype, [&](auto dt) {
+    constexpr int DT = decltype(dt)::value;
+    if (cwa == 64 && na == 2) return launch_wgrad2<64, 2, 16, DT>(mdy, mx0, mx1, p, m_tiles, stream);
+    if (cwa == 64) return launch_wgrad2<64, 1, 16, DT>(mdy, mx0, mx1, p, m_tiles, stream);
+    if (cwa == 32) return launch_wgrad2<32, 1, 16, DT>(mdy, mx0, mx1, p, m_tiles, stream);
+    return launch_wgrad2<16, 1, 16, DT>(mdy, mx0, mx1, p, m_tiles, stream);
+  });
 }
 
 // 3x3 weight gradient, v3 (filter columns in the MMA's M dimension).  Same contract as wsl_wgrad_tc2.
@@ -1802,12 +1858,15 @@ WSL_API int wsl_wgrad_tc3(const void* src0, int C0, const void* src1, int C1, co
   p.N = N; p.H = H; p.W = W; p.C0 = C0; p.C1 = C1; p.CoutReal = CoutReal;
   p.tiles_x = W / 8; p.tiles_y = H / 16; p.nchunks = N * p.tiles_x * p.tiles_y;
   p.k_tiles0 = C0 / cwb; p.k_tiles1 = C1 / cwb; p.dt = dtype; p.dw = dw; p.partials = nullptr;
+  return with_dt(dtype, [&](auto dt) {
+    constexpr int DT = decltype(dt)::value;
 #define WSL_W3(CWB_) \
-  if (ntile == 64) return launch_wgrad3<CWB_, 64>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);  \
-  if (ntile == 32) return launch_wgrad3<CWB_, 32>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);  \
-  return launch_wgrad3<CWB_, 16>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);
-  if (cwb == 32) { WSL_W3(32) }
-  WSL_W3(16)
+    if (ntile == 64) return launch_wgrad3<CWB_, 64, DT>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);  \
+    if (ntile == 32) return launch_wgrad3<CWB_, 32, DT>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);  \
+    return launch_wgrad3<CWB_, 16, DT>(mdy, mx0, mx1, p, n_tiles, partial_ws, partial_floats, stream);
+    if (cwb == 32) { WSL_W3(32) }
+    WSL_W3(16)
 #undef WSL_W3
+  });
 }
 
