@@ -173,6 +173,21 @@ int wsl_random_walker(const float* images, const uint8_t* scribbles, const long 
                       int n_slices, float beta, float tol, int max_iter, float* ws, int ctas, long long slot_px, uint8_t* labels,
                       float* probs, int* iters, float* resid, cudaStream_t stream);
 
+/* Surface metrics of two uint8 label volumes pred / gt, [S,H,W] (ndim 3) or [H,W] (ndim 2, S = 1), for classes 1..classes-1
+ * (2 <= classes <= 16, W <= 4096, at most 2^30 voxels): medpy.metric.binary dc / jc / hd95 / asd with voxelspacing (sz, sy, sx; sz unused for ndim 2)
+ * and connectivity 1, i.e. its __surface_distances as val_2D.py:7-15 (calculate_metric_percase), test_2D_fully.py:74-80 and
+ * utils/metrics.py:19-25 call it: surface = mask ^ binary_erosion(mask, generate_binary_structure(ndim, 1)) (border voxels are
+ * surface, so a [1,H,W] volume differs from its [H,W] slice), distances = distance_transform_edt(~surface, sampling) at the other
+ * surface, exact, fp64, evaluated as scipy does.  out: (classes-1) rows of 12 doubles,
+ *   {|P&G|, |P|, |G|, |P|G|, nA, nB, sumA, sumB, maxA, maxB, x[lo], x[hi]},
+ * A = pred-surface -> gt-surface distances (asd = sumA / nA), B = gt -> pred, x[lo] / x[hi] the order statistics at
+ * lo = floor((n-1)*0.95), hi = lo + 1 (both n-1 at the top) of the n = nA + nB distances of both directions, which
+ * np.percentile(.., 95) interpolates.  A class whose pred or gt mask is empty keeps 0 in fields 6..11.  Sums are in a fixed
+ * order (bit-identical run to run).  ws: wsl_surface_metrics_workspace() bytes, 256-byte aligned, no zeroing needed; out_bytes is a HOST pointer. */
+int wsl_surface_metrics_workspace(int ndim, int S, int H, int W, int classes, long long* out_bytes);
+int wsl_surface_metrics(const uint8_t* pred, const uint8_t* gt, int ndim, int S, int H, int W, int classes, double sz, double sy,
+                        double sx, void* ws, double* out, cudaStream_t stream);
+
 /* ---- network operators (networks/unet.py) ---------------------------------------------------------------- */
 
 /* nn.Conv2d(k=3,pad=1)/(k=1) forward on CUDA cores (unet.py:19,23,55,120); with dgrad-packed weights also the

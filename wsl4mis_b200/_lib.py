@@ -17,6 +17,7 @@ LIB_PATH = os.path.join(PKG, "libwsl4mis_b200.so")
 _SCALARS = {
     "int": ctypes.c_int,
     "float": ctypes.c_float,
+    "double": ctypes.c_double,
     "long long": ctypes.c_longlong,
     "unsigned long long": ctypes.c_ulonglong,
     "unsigned int": ctypes.c_uint,

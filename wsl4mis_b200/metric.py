@@ -1,0 +1,139 @@
+"""medpy.metric.binary's ``dc`` / ``jc`` / ``hd95`` / ``asd`` on the GPU, and ``surface_metrics``, the per-volume form over label
+maps that the validation pass uses (val_2D.py:7-15, test_2D_fully.py:74-80, utils/metrics.py:19-25).
+
+Surfaces, the exact anisotropic distance transforms and the order statistics of HD95 run in csrc/metrics.cu; one small
+device-to-host copy brings back a few doubles per class.  The last step of ``np.percentile`` (numpy's ``_lerp`` between the two
+order statistics) is done here in the same float64 arithmetic, so HD95 equals medpy's value bit for bit wherever the distances do
+(unit and integer spacings).
+"""
+import ctypes
+from typing import NamedTuple
+
+import numpy as np
+import torch
+
+from ._lib import call
+
+
+class SurfaceMetrics(NamedTuple):
+    """Per class: overlap counts and the surface-distance metrics.  hd95 / asd are nan when either mask is empty (medpy raises
+    there; each caller applies its own rule from the counts)."""
+    inter: int
+    pred: int
+    gt: int
+    union: int
+    hd95: float
+    asd: float
+
+
+def _spacing(voxelspacing, ndim):
+    """scalar or one value per axis -> ndim floats (medpy's _ni_support._normalize_sequence)."""
+    if voxelspacing is None:
+        return (1.0,) * ndim
+    sp = np.asarray(voxelspacing, dtype=np.float64)
+    if sp.ndim == 0:
+        return (float(sp),) * ndim
+    if sp.shape != (ndim,):
+        raise RuntimeError("sequence argument must have length equal to input rank")
+    return tuple(float(v) for v in sp)
+
+
+def _percentile95(lo, hi, n):
+    """np.percentile(x, 95) from its two order statistics x[lo] <= x[hi] ('linear' method, numpy's _lerp)."""
+    vi = (n - 1) * 0.95
+    if vi >= n - 1:
+        return hi
+    g = vi - float(np.floor(vi))
+    d = hi - lo
+    return hi - d * (1 - g) if g >= 0.5 else lo + d * g
+
+
+def _device_mask(x, device=None):
+    """numpy array or tensor -> contiguous CUDA uint8 0/1 mask, nonzero = 1 (medpy's astype(bool)), compared in the input's own
+    dtype so that 0.5 or 256 count as True."""
+    m = (x != 0) if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(np.asarray(x) != 0))
+    dev = device or (m.device if m.is_cuda else "cuda")
+    return m.to(device=dev, dtype=torch.uint8).contiguous()
+
+
+def surface_metrics(pred, gt, classes, voxelspacing=None):
+    """Counts, hd95 and asd of every class 1..classes-1 of two uint8 label volumes ([S,H,W] or [H,W], CUDA tensors) in one
+    kernel sequence.  Returns [SurfaceMetrics] indexed by class - 1."""
+    if pred.shape != gt.shape:
+        raise ValueError(f"surface_metrics: shape mismatch {tuple(pred.shape)} vs {tuple(gt.shape)}")
+    if pred.dim() not in (2, 3):
+        raise ValueError(f"surface_metrics: volumes must have rank 2 or 3 (got {pred.dim()})")
+    if not (pred.is_cuda and gt.is_cuda and pred.device == gt.device) or pred.dtype != torch.uint8 or gt.dtype != torch.uint8:
+        raise ValueError("surface_metrics: pred and gt must be uint8 tensors on the same CUDA device")
+    ndim = pred.dim()
+    S, H, W = ((1,) + tuple(pred.shape)) if ndim == 2 else tuple(pred.shape)
+    sp = _spacing(voxelspacing, ndim)
+    sz, sy, sx = ((1.0,) + sp) if ndim == 2 else sp
+    with torch.cuda.device(pred.device):
+        nbytes = ctypes.c_longlong(0)
+        call("wsl_surface_metrics_workspace", ndim, S, H, W, classes, ctypes.addressof(nbytes))
+        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=pred.device)
+        out = torch.empty((classes - 1, 12), dtype=torch.float64, device=pred.device)
+        call("wsl_surface_metrics", pred.contiguous(), gt.contiguous(), ndim, S, H, W, classes, sz, sy, sx, ws, out)
+        o = out.cpu().numpy()
+    res = []
+    for r in o:
+        inter, npred, ngt, union, na, nb = (int(v) for v in r[:6])
+        if npred and ngt:
+            hd, asd = float(_percentile95(float(r[10]), float(r[11]), na + nb)), float(r[6] / na)
+        else:
+            hd = asd = float("nan")
+        res.append(SurfaceMetrics(inter, npred, ngt, union, hd, asd))
+    return res
+
+
+def _binary(result, reference, voxelspacing, connectivity):
+    if connectivity != 1:
+        raise NotImplementedError("only connectivity=1 (face neighbours), the value every caller uses, is implemented")
+    a = _device_mask(result)
+    b = _device_mask(reference, a.device)
+    if a.shape != b.shape:
+        raise ValueError(f"shape mismatch {tuple(a.shape)} vs {tuple(b.shape)}")
+    m = surface_metrics(a, b, 2, voxelspacing)[0]
+    if m.pred == 0:
+        raise RuntimeError('The first supplied array does not contain any binary object.')
+    if m.gt == 0:
+        raise RuntimeError('The second supplied array does not contain any binary object.')
+    return m
+
+
+def _counts(result, reference):
+    a = _device_mask(result)
+    b = _device_mask(reference, a.device)
+    if a.shape != b.shape:
+        raise ValueError(f"shape mismatch {tuple(a.shape)} vs {tuple(b.shape)}")
+    counts = torch.zeros(6, dtype=torch.int64, device=a.device)
+    with torch.cuda.device(a.device):
+        call("wsl_overlap_counts", a, b, a.numel(), 2, counts)
+        inter, sa, sb = (int(v) for v in counts[3:].cpu())
+    return inter, sa, sb
+
+
+def dc(result, reference):
+    """Dice coefficient 2|A&B| / (|A| + |B|), 0.0 when both are empty (medpy.metric.binary.dc)."""
+    inter, sa, sb = _counts(result, reference)
+    try:
+        return 2.0 * inter / float(sa + sb)
+    except ZeroDivisionError:
+        return 0.0
+
+
+def jc(result, reference):
+    """Jaccard coefficient |A&B| / |A|B| (medpy.metric.binary.jc)."""
+    inter, sa, sb = _counts(result, reference)
+    return float(inter) / float(sa + sb - inter)
+
+
+def hd95(result, reference, voxelspacing=None, connectivity=1):
+    """95th percentile of the symmetric surface distances (medpy.metric.binary.hd95)."""
+    return _binary(result, reference, voxelspacing, connectivity).hd95
+
+
+def asd(result, reference, voxelspacing=None, connectivity=1):
+    """Mean distance of the surface of `result` to the surface of `reference` (medpy.metric.binary.asd)."""
+    return _binary(result, reference, voxelspacing, connectivity).asd

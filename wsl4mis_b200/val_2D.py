@@ -3,13 +3,15 @@
 The reference loops over the slices of a volume on the host: scipy ``zoom(order=0)`` to 256x256, a batch-1 forward,
 argmax, ``zoom`` back, then medpy Dice / HD95 per class.  Here all slices of the volume go through the network as one
 batch; both nearest-neighbour resizes, the argmax and the Dice overlap counts run on the GPU (SciPy's index rule is
-reproduced bit for bit, see csrc/losses.cu).  HD95 stays on the host like in the reference (scipy distance transform;
-medpy is not a dependency).
+reproduced bit for bit, see csrc/losses.cu).  HD95 too: surfaces, exact distance transforms and the percentile's order
+statistics run in csrc/metrics.cu (``metric.surface_metrics``), one call per volume.  ``hd95`` / ``calculate_metric_percase``
+below keep medpy's host algorithm on scipy (medpy is not a dependency) as the reference the GPU path is tested against.
 """
 import numpy as np
 import torch
 
 from ._lib import call
+from .metric import surface_metrics
 
 
 def _surface_distances(result, reference):
@@ -54,18 +56,13 @@ def _predict_volume(image, net, patch_size, head):
 
 
 def _metrics(pred, label, classes):
-    dev = pred.device
-    gt = torch.as_tensor(np.ascontiguousarray(label)).to(device=dev, dtype=torch.uint8)
-    counts = torch.zeros(classes * 3, dtype=torch.int64, device=dev)
-    call("wsl_overlap_counts", pred.contiguous(), gt.contiguous(), pred.numel(), classes, counts)
-    c = counts.cpu().numpy().reshape(classes, 3)
-    pred_h, gt_h = pred.cpu().numpy(), gt.cpu().numpy()
+    gt = torch.as_tensor(np.ascontiguousarray(label)).to(device=pred.device, dtype=torch.uint8)
     out = []
-    for i in range(1, classes):
-        inter, sp, sg = int(c[i, 0]), int(c[i, 1]), int(c[i, 2])
-        if sp > 0:   # calculate_metric_percase (val_2D.py:7-15): (0, 0) when the prediction is empty
-            dice = 2.0 * inter / float(sp + sg)
-            out.append((dice, hd95(pred_h == i, gt_h == i)))
+    for m in surface_metrics(pred.contiguous(), gt.contiguous(), classes):
+        if m.pred > 0:   # calculate_metric_percase (val_2D.py:7-15): (0, 0) when the prediction is empty
+            if m.gt == 0:
+                raise RuntimeError('The second supplied array does not contain any binary object.')
+            out.append((2.0 * m.inter / float(m.pred + m.gt), m.hd95))
         else:
             out.append((0, 0))
     return out
