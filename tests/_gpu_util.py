@@ -53,6 +53,32 @@ def pack_conv_weights(w, c_slices, dt=0):
     return pk
 
 
+class LaunchRecorder:
+    """Stands in for wsl4mis_b200._lib.PROFILE: runs every C-ABI call as call() does (a nonzero return code raises) and keeps the
+    distinct launches whose entry point `keep(name)` accepts, as (entry, ((scalar name, value), ...), (names of pointer arguments
+    passed as NULL, ...)) -> number of calls.  on_record(key, name, vals), when given, sees every kept call (pointer values included)."""
+
+    def __init__(self, keep, on_record=None):
+        self.meta = None
+        self.keep = keep
+        self.on_record = on_record
+        self.launches = {}
+
+    def record(self, name, fn, vals):
+        import ctypes
+        from wsl4mis_b200._lib import LIB
+        rc = fn(*vals)
+        if rc != 0:
+            raise RuntimeError(f"{name} failed ({rc}): {LIB.last_error()}")
+        if self.keep(name):
+            args = [(nm, ty, v) for (ty, nm), v in zip(LIB.protos[name][1], vals) if nm != "stream"]
+            key = (name, tuple((nm, v) for nm, ty, v in args if ty is not ctypes.c_void_p),
+                   tuple(nm for nm, ty, v in args if ty is ctypes.c_void_p and v is None))
+            self.launches[key] = self.launches.get(key, 0) + 1
+            if self.on_record is not None:
+                self.on_record(key, name, vals)
+
+
 def rel_l2(a, b):
     a, b = a.double().flatten(), b.double().flatten()
     return ((a - b).norm() / (b.norm() + 1e-30)).item()

@@ -20,14 +20,14 @@ import pytest
 import torch
 
 import _conv_check as CC
-from _gpu_util import pack_conv_weights
+from _gpu_util import LaunchRecorder, pack_conv_weights
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
 if torch.cuda.is_available():
     from wsl4mis_b200 import _lib
-    from wsl4mis_b200._lib import LIB, call
+    from wsl4mis_b200._lib import call
     from wsl4mis_b200.networks.pnet import PNet2D
     from wsl4mis_b200.networks.unet import UNet_CCT
 
@@ -49,32 +49,13 @@ CONFIGS = {
 _RESULTS = {}
 
 
-class LaunchRecorder:
-    """Stands in for _lib.PROFILE: runs every C-ABI call as call() does (a nonzero return code raises) and keeps the distinct
-    harvested launches as (entry, ((scalar name, value), ...), (names of pointer arguments passed as NULL, ...))."""
-
-    def __init__(self):
-        self.meta = None
-        self.launches = {}
-
-    def record(self, name, fn, vals):
-        rc = fn(*vals)
-        if rc != 0:
-            raise RuntimeError(f"{name} failed ({rc}): {LIB.last_error()}")
-        if name in HARVESTED:
-            args = [(nm, ty, v) for (ty, nm), v in zip(LIB.protos[name][1], vals) if nm != "stream"]
-            key = (name, tuple((nm, v) for nm, ty, v in args if ty is not ctypes.c_void_p),
-                   tuple(nm for nm, ty, v in args if ty is ctypes.c_void_p and v is None))
-            self.launches[key] = self.launches.get(key, 0) + 1
-
-
 def _harvest(model, N, precision):
     torch.manual_seed(0)
     m = UNet_CCT(1, 4) if model == "unet_cct" else PNet2D(1, 4, 64, [1, 2, 4, 8, 16])
     m = m.to(DEV).set_precision(precision)
     m.train()
     x = torch.rand(N, 1, 256, 256, device=DEV)
-    rec, saved = LaunchRecorder(), _lib.PROFILE
+    rec, saved = LaunchRecorder(lambda name: name in HARVESTED), _lib.PROFILE
     _lib.PROFILE = rec
     try:
         out = m(x)
