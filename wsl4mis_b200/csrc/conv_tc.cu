@@ -72,6 +72,28 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* ba
       ::"r"(smem_u32(dst)), "l"((uint64_t)map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// TMA tensor store from shared memory, tracked by the issuing thread's bulk async-groups; out-of-bounds parts of the box
+// are not written.  Shared-memory writes of other threads must be made visible to the async proxy first (fence_proxy_async
+// by every writer, then a barrier).  These run only where `on` is set, as predicated instructions: a branch on the thread
+// index while an MMA group is in flight makes ptxas serialise every wgmma of the kernel (C7518).
+__device__ __forceinline__ void tma_store_4d(bool on, const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %0, 0;\n\t"
+               "@p cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%1, {%3, %4, %5, %6}], [%2];\n\t}"
+               ::"r"((uint32_t)on), "l"((uint64_t)map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit(bool on) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %0, 0;\n\t@p cp.async.bulk.commit_group;\n\t}" ::"r"((uint32_t)on) : "memory");
+}
+// every committed store has finished reading its shared-memory source (the buffer may be overwritten)
+__device__ __forceinline__ void bulk_wait_read_all(bool on) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %0, 0;\n\t@p cp.async.bulk.wait_group.read 0;\n\t}" ::"r"((uint32_t)on) : "memory");
+}
+// every committed store has completed
+__device__ __forceinline__ void bulk_wait_all(bool on) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %0, 0;\n\t@p cp.async.bulk.wait_group 0;\n\t}" ::"r"((uint32_t)on) : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
 }
@@ -390,14 +412,54 @@ struct ConvV2Cfg {
   static constexpr int HALO_BYTES = HW_ * HH_ * ROWB;
   static constexpr int A_STAGE = ((HALO_BYTES + 1023) / 1024) * 1024;
   static constexpr int W_SUB = NT * ROWB;                  // one (tap, k-block) weight tile
+  // 16-bit output tile staged for the TMA store: OUT_BOXES boxes of OUT_CH channels x 8 w x TH h, each in the swizzle of
+  // its OUT_CH * 2-byte rows (so the epilogue's writes, 8 pixels x 4 channel pairs per warp instruction, hit 32 banks)
+  static constexpr int OUT_CH = NT < 64 ? NT : 64, OUT_BOXES = NT / OUT_CH;
+  static constexpr int OUT_BOX_BYTES = TW * TH * OUT_CH * 2, OUT_BYTES = OUT_BOXES * OUT_BOX_BYTES;
 };
+
+// Byte offset of (pixel px of the tile, channel c of the N tile) in the staged output tile: box c / OUT_CH, row px, in the
+// TMA swizzle of the box (16-byte chunk index XOR row-of-128-bytes index, over OUT_CH * 2 / 16 chunks).
+template <int OUT_CH, int OUT_BOX_BYTES>
+__device__ __forceinline__ uint32_t out_stage_offset(int px, int c) {
+  constexpr uint32_t ROWB = OUT_CH * 2, CHUNK_MASK = ROWB / 16 - 1;
+  const uint32_t o = (uint32_t)px * ROWB + (uint32_t)(c % OUT_CH) * 2;
+  return (uint32_t)(c / OUT_CH) * OUT_BOX_BYTES + (o ^ (((o >> 7) & CHUNK_MASK) << 4));
+}
+
+// The MMAs of k-block kb of one tile (MT sub-tiles x T taps x KBLK/16 k-steps) as one commit group.  The first MMA of each
+// sub-tile at kb = 0 has scale-d = 0, so acc needs no zero fill: no other instruction writes accumulator registers while the
+// previous tile's epilogue runs under this group.
+template <int KS, int KBLK, int NT, int MT, int DT>
+__device__ __forceinline__ void tile_mma(float (&acc)[MT][NT / 2], uint32_t a_base, uint32_t w_base, int kb, int nkb) {
+  using Cfg = ConvV2Cfg<KS, KBLK, NT, MT>;
+  constexpr int SW = KBLK * 2, T = KS * KS;
+  // The next tile's first group reads the loop-invariant weight slice: without this, ptxas hoists its T * KBLK / 16 64-bit
+  // descriptors out of the tile loop and keeps them live (spilling) across the whole epilogue.
+  asm volatile("" : "+r"(w_base));
+  wgmma_fence();
+#pragma unroll
+  for (int j = 0; j < MT; ++j) {
+#pragma unroll
+    for (int tap = 0; tap < T; ++tap) {
+      const int dy = tap / KS, dx = tap % KS;
+#pragma unroll
+      for (int k = 0; k < KBLK / 16; ++k)
+        Wgmma<NT>::template mma<0, 0, DT>(acc[j],
+                                          gmma_desc<SW>(a_base + (uint32_t)(((16 * j + dy) * Cfg::HW_ + dx) * Cfg::ROWB + 32 * k), 16, Cfg::HW_ * Cfg::ROWB),
+                                          gmma_desc<SW>(w_base + (uint32_t)(tap * nkb * Cfg::W_SUB + 32 * k), 16, 8 * SW),
+                                          (kb > 0 || tap > 0 || k > 0) ? 1u : 0u);
+    }
+  }
+  wgmma_commit();
+}
 
 // Per-thread running BatchNorm sums (NT/4 channels per thread: column 8*j + frag_col + b) -> this CTA's row of
 // stat_partials: the lanes holding the same channels are summed with shuffles, then the eight consumer warps in a
-// fixed order.  Consumer threads only (named barrier 1).
+// fixed order.  Consumer threads only (named barrier 1); s_stat is shared-memory scratch of the caller.
 template <int NT>
-__device__ __forceinline__ void write_stat_partials(float (&rs)[NT / 4], float (&rq)[NT / 4], float* stat_partials, int CoutP, int n0) {
-  __shared__ float s_stat[CONSUMER_WARPS][2][NT];
+__device__ __forceinline__ void write_stat_partials(float (&rs)[NT / 4], float (&rq)[NT / 4], float* stat_partials, int CoutP, int n0,
+                                                    float (*s_stat)[2][NT]) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 #pragma unroll
   for (int k = 0; k < NT / 4; ++k) {
@@ -428,16 +490,18 @@ __device__ __forceinline__ void write_stat_partials(float (&rs)[NT / 4], float (
 template <int KS, int KBLK, int NT, int MT, int STAGES, int DT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc2_kernel(const __grid_constant__ CUtensorMap map_a0,
                                                                   const __grid_constant__ CUtensorMap map_a1,
-                                                                  const __grid_constant__ CUtensorMap map_b, const ConvV2Params p,
+                                                                  const __grid_constant__ CUtensorMap map_b,
+                                                                  const __grid_constant__ CUtensorMap map_o, const ConvV2Params p,
                                                                   const int w_bytes) {
   using Cfg = ConvV2Cfg<KS, KBLK, NT, MT>;
-  constexpr int SW = KBLK * 2, T = KS * KS;
+  constexpr int T = KS * KS;
   static_assert(MT * NT <= 128, "accumulator registers");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* w_smem = smem;
   uint8_t* a_smem = smem + w_bytes;                         // w_bytes is a multiple of 1024
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + STAGES * Cfg::A_STAGE);
+  uint8_t* o_smem = a_smem + STAGES * Cfg::A_STAGE;         // staged 16-bit output tile (1024-aligned: the swizzle atom)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(o_smem + Cfg::OUT_BYTES);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + STAGES;
   uint64_t* w_bar = bars + 2 * STAGES;
@@ -453,6 +517,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc2_kernel(const __grid_c
     fence_barrier_init();
     prefetch_tmap(&map_a0);
     prefetch_tmap(&map_b);
+    if (p.out_mode == 0) prefetch_tmap(&map_o);
   }
   __syncthreads();
 
@@ -486,69 +551,137 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc2_kernel(const __grid_c
   float rs[NT / 4], rq[NT / 4];          // running per-channel sum / sum of squares of this thread's pixels
 #pragma unroll
   for (int k = 0; k < NT / 4; ++k) rs[k] = rq[k] = 0.f;
+  __shared__ float s_bias[NT];
+  if (threadIdx.x < NT) s_bias[threadIdx.x] = p.bias ? p.bias[n0 + threadIdx.x] : 0.f;
+  asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+  const bool store_thread = threadIdx.x == 0;   // issues (and waits for) the TMA stores of the output tiles
+  const bool stats = p.out_mode == 0 && p.stat_partials;
   mbar_wait(w_bar, 0);
-  int it = 0;
-  for (int i = 0; i < my_tiles; ++i) {
+  // One MMA group in flight: group `it` reads A stage it % STAGES and is released once the next group has been issued and
+  // it has retired (the same stage order as a serial tile loop).  Tile i + 1's first group is issued as soon as tile i's
+  // accumulator is rounded into registers, so tile i's BatchNorm sums and stores run under it.  Rows 64h.. of a sub-tile
+  // start 8h halo rows further down.
+  const uint32_t a_h = a_u + (uint32_t)(8 * h * Cfg::HW_ * Cfg::ROWB);
+  float acc[MT][NT / 2];
+  // 16-bit NHWC epilogue.  stage_tile rounds each channel pair (c, c + 1) of pixel m to the 16-bit type (value(j, ii, jj)),
+  // accumulates the BatchNorm sums of the rounded values and writes them to the staging buffer; store_tile hands the buffer
+  // to TMA.  When the registers allow, the tile is first rounded into pk (registers no MMA writes) and both run under the
+  // next tile's first MMA group: pk (a quarter of MT * NT) and the running sums (NT / 2) then live beside the in-flight
+  // accumulator (MT * NT / 2).  ptxas allocates the 168 registers of a 384-thread CTA (the setmaxnreg raise to 232 does not
+  // enter its allocation), so larger tiles are staged straight from the accumulator before the group is issued and only the
+  // store overlaps.
+  constexpr bool STAGE_UNDER_MMA = 3 * MT * NT / 4 + NT / 2 <= 64;
+  // staging offset of this thread's first pair: pixel 64h + frag_row, channel frag_col
+  const uint32_t o_thr = out_stage_offset<Cfg::OUT_CH, Cfg::OUT_BOX_BYTES>(64 * h + frag_row(t), frag_col(t));
+  auto stage_tile = [&](auto&& value) {
+    bulk_wait_read_all(store_thread);       // the previous tile's store has read the staging buffer
+    asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+#pragma unroll
+    for (int j = 0; j < MT; ++j)
+#pragma unroll
+      for (int ii = 0; ii < 2; ++ii)
+#pragma unroll
+        for (int jj = 0; jj < NT / 8; ++jj) {
+          const uint32_t u = value(j, ii, jj);
+          if (stats) {                      // BatchNorm statistics of the values exactly as stored
+            float2 r;
+            if (DT == 2) r = __half22float2(*reinterpret_cast<const __half2*>(&u));
+            else r = make_float2(bf16_lo(u), bf16_hi(u));
+            rs[2 * jj] += r.x;     rq[2 * jj] += r.x * r.x;
+            rs[2 * jj + 1] += r.y; rq[2 * jj + 1] += r.y * r.y;
+          }
+          // pixel 128 j + 8 ii further on is a multiple of 256 bytes further on, which keeps the swizzle phase: the 16-byte
+          // chunk of channel group jj is an XOR of the thread's base offset (one live register, no per-chunk addresses)
+          constexpr int CG = Cfg::OUT_CH / 8;
+          const uint32_t off = (o_thr + (uint32_t)((jj / CG) * Cfg::OUT_BOX_BYTES + (128 * j + 8 * ii) * Cfg::OUT_CH * 2)) ^ (uint32_t)((jj % CG) << 4);
+          *reinterpret_cast<uint32_t*>(o_smem + off) = u;
+        }
+    fence_proxy_async();
+  };
+  auto store_tile = [&](int n, int y0, int x0) {
+    asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+#pragma unroll
+    for (int b = 0; b < Cfg::OUT_BOXES; ++b)
+      tma_store_4d(store_thread, &map_o, o_smem + b * Cfg::OUT_BOX_BYTES, n0 + b * Cfg::OUT_CH, x0, y0, n);
+    bulk_commit(store_thread);
+  };
+  auto from_acc = [&](int j, int ii, int jj) -> uint32_t {
+    const int c = 8 * jj + frag_col(t);
+    float v0 = acc[j][4 * jj + 2 * ii], v1 = acc[j][4 * jj + 2 * ii + 1];
+    if (p.bias) { v0 += s_bias[c]; v1 += s_bias[c + 1]; }
+    return DT == 2 ? pack_f16(v0, v1) : pack_bf16(v0, v1);
+  };
+  // Every CTA has at least one tile (the host keeps the grid <= ntiles), so the first group is issued unconditionally: the
+  // MMAs are issued on paths that never join one without a group in flight (a join of the two makes ptxas serialise, C7518).
+  mbar_wait(&a_full[0], 0);
+  tile_mma<KS, KBLK, NT, MT, DT>(acc, a_h, w_u, 0, nkb);
+  int it = 1;
+  for (int i = 0;; ++i) {
     const int tile = blockIdx.x + i * gridDim.x;
     const int n = tile / (p.tiles_x * p.tiles_y);
     const int tr = tile - n * p.tiles_x * p.tiles_y;
     const int y0 = (tr / p.tiles_x) * Cfg::TH, x0 = (tr % p.tiles_x) * Cfg::TW;
-    float acc[MT][NT / 2];
-#pragma unroll
-    for (int j = 0; j < MT; ++j)
-#pragma unroll
-      for (int e = 0; e < NT / 2; ++e) acc[j][e] = 0.f;
-    for (int kb = 0; kb < nkb; ++kb, ++it) {
+    for (int kb = 1; kb < nkb; ++kb, ++it) {
       const int s = it % STAGES;
       mbar_wait(&a_full[s], (it / STAGES) & 1);
-      // rows 64h.. of a sub-tile start 8h halo rows further down
-      const uint32_t a_base = a_u + (uint32_t)(s * Cfg::A_STAGE + 8 * h * Cfg::HW_ * Cfg::ROWB);
-      const uint32_t w_base = w_u + (uint32_t)(kb * Cfg::W_SUB);
-      wgmma_fence();
-#pragma unroll
-      for (int j = 0; j < MT; ++j) {
-#pragma unroll
-        for (int tap = 0; tap < T; ++tap) {
-          const int dy = tap / KS, dx = tap % KS;
-#pragma unroll
-          for (int k = 0; k < KBLK / 16; ++k)
-            Wgmma<NT>::template mma<0, 0, DT>(acc[j],
-                                              gmma_desc<SW>(a_base + (uint32_t)(((16 * j + dy) * Cfg::HW_ + dx) * Cfg::ROWB + 32 * k), 16, Cfg::HW_ * Cfg::ROWB),
-                                              gmma_desc<SW>(w_base + (uint32_t)(tap * nkb * Cfg::W_SUB + 32 * k), 16, 8 * SW),
-                                              (kb > 0 || tap > 0 || k > 0) ? 1u : 0u);
-        }
-      }
-      wgmma_commit();
+      tile_mma<KS, KBLK, NT, MT, DT>(acc, a_h + (uint32_t)(s * Cfg::A_STAGE), w_u + (uint32_t)(kb * Cfg::W_SUB), kb, nkb);
       wgmma_wait<1>();                     // the previous k-block's group has retired: its stage can be refilled
-      if (kb > 0) release_stage(&a_empty[(it + STAGES - 1) % STAGES]);
+      release_stage(&a_empty[(it + STAGES - 1) % STAGES]);
     }
     wgmma_wait<0>();
     release_stage(&a_empty[(it + STAGES - 1) % STAGES]);
 #pragma unroll
-    for (int j = 0; j < MT; ++j) {
-      wgmma_fence_regs(acc[j]);
+    for (int j = 0; j < MT; ++j) wgmma_fence_regs(acc[j]);
+    uint32_t pk[MT][2][NT / 8];
+    if (p.out_mode == 0) {
+      if constexpr (STAGE_UNDER_MMA) {
 #pragma unroll
-      for (int ii = 0; ii < 2; ++ii) {
-        const int m = 64 * h + frag_row(t) + 8 * ii;
-        const int gy = y0 + 16 * j + m / 8, gx = x0 + (m & 7);
+        for (int j = 0; j < MT; ++j)
 #pragma unroll
-        for (int jj = 0; jj < NT / 8; ++jj) {
-          const int c = 8 * jj + frag_col(t);
-          float v0 = acc[j][4 * jj + 2 * ii], v1 = acc[j][4 * jj + 2 * ii + 1];
-          if (p.bias) { v0 += p.bias[n0 + c]; v1 += p.bias[n0 + c + 1]; }
-          if (p.out_mode == 0 && p.stat_partials) {   // BatchNorm statistics of the values exactly as stored
-            float2 r;
-            if (DT == 2) r = __half22float2(__floats2half2_rn(v0, v1));
-            else r = __bfloat1622float2(__floats2bfloat162_rn(v0, v1));
-            rs[2 * jj] += r.x;     rq[2 * jj] += r.x * r.x;
-            rs[2 * jj + 1] += r.y; rq[2 * jj + 1] += r.y * r.y;
-          }
-          store_pair(p.out, p.out_mode == 0 ? 0 : 1, DT, p.CoutStore, p.H, p.W, n, gy, gx, n0 + c, v0, v1);
-        }
+          for (int ii = 0; ii < 2; ++ii)
+#pragma unroll
+            for (int jj = 0; jj < NT / 8; ++jj) pk[j][ii][jj] = from_acc(j, ii, jj);
+      } else {
+        stage_tile(from_acc);
       }
+    } else {                                // fp32 NCHW (the logits): stored from the accumulator before the next group
+#pragma unroll
+      for (int j = 0; j < MT; ++j)
+#pragma unroll
+        for (int ii = 0; ii < 2; ++ii) {
+          const int m = 64 * h + frag_row(t) + 8 * ii;
+          const int gy = y0 + 16 * j + m / 8, gx = x0 + (m & 7);
+#pragma unroll
+          for (int jj = 0; jj < NT / 8; ++jj) {
+            const int c = 8 * jj + frag_col(t);
+            float v0 = acc[j][4 * jj + 2 * ii], v1 = acc[j][4 * jj + 2 * ii + 1];
+            if (p.bias) { v0 += s_bias[c]; v1 += s_bias[c + 1]; }
+            store_pair(p.out, 1, DT, p.CoutStore, p.H, p.W, n, gy, gx, n0 + c, v0, v1);
+          }
+        }
     }
+#pragma unroll
+    for (int j = 0; j < MT; ++j) wgmma_discard_regs(acc[j]);
+    auto finish_tile = [&]() {
+      if (p.out_mode == 0) {
+        if constexpr (STAGE_UNDER_MMA) stage_tile([&](int j, int ii, int jj) { return pk[j][ii][jj]; });
+        store_tile(n, y0, x0);
+      }
+    };
+    if (i + 1 == my_tiles) {                // last tile: no next group to overlap
+      finish_tile();
+      break;
+    }
+    mbar_wait(&a_full[it % STAGES], (it / STAGES) & 1);
+    tile_mma<KS, KBLK, NT, MT, DT>(acc, a_h + (uint32_t)((it % STAGES) * Cfg::A_STAGE), w_u, 0, nkb);
+    ++it;
+    finish_tile();
   }
-  if (p.out_mode == 0 && p.stat_partials) write_stat_partials<NT>(rs, rq, p.stat_partials, p.CoutP, n0);
+  bulk_wait_all(store_thread);
+  if (stats) {                              // the staging buffer is free: it holds the cross-warp combine
+    asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+    write_stat_partials<NT>(rs, rq, p.stat_partials, p.CoutP, n0, reinterpret_cast<float (*)[2][NT]>(o_smem));
+  }
 }
 
 // ================================================================================================
@@ -1188,13 +1321,14 @@ __global__ void __launch_bounds__(256) channel_sum_kernel(const T* __restrict__ 
 static int g_conv2_last_rows = 0;   // gridDim.x of the most recent conv_tc2 launch (rows of stat_partials)
 
 template <int KS, int KBLK, int NT, int MT, int DT>
-int launch_conv2(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, cudaStream_t stream) {
+int launch_conv2(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& o, const ConvV2Params& p,
+                 cudaStream_t stream) {
   using Cfg = ConvV2Cfg<KS, KBLK, NT, MT>;
   constexpr int STAGES = (Cfg::A_STAGE <= 8 * 1024) ? 4 : (Cfg::A_STAGE <= 13 * 1024) ? 3 : 2;
   const int T = KS * KS;
   const int nkb = (p.C0 + p.C1) / KBLK;
   const int w_bytes = ((T * nkb * Cfg::W_SUB + 1023) / 1024) * 1024;
-  const int smem = w_bytes + STAGES * Cfg::A_STAGE + 1024 + 256;
+  const int smem = w_bytes + STAGES * Cfg::A_STAGE + Cfg::OUT_BYTES + 1024 + 256;
   if (smem > 227 * 1024) { wsl_set_error("conv_tc2: %d bytes of shared memory needed", smem); return -6; }
   static int attr_bytes = 0;
   if (smem > attr_bytes) {
@@ -1211,19 +1345,20 @@ int launch_conv2(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap
   if (gx > p.ntiles) gx = p.ntiles;
   dim3 grid(gx, n_tiles);
   g_conv2_last_rows = gx;
-  conv_tc2_kernel<KS, KBLK, NT, MT, STAGES, DT><<<grid, NUM_THREADS, smem, stream>>>(a0, a1, b, p, w_bytes);
+  conv_tc2_kernel<KS, KBLK, NT, MT, STAGES, DT><<<grid, NUM_THREADS, smem, stream>>>(a0, a1, b, o, p, w_bytes);
   return wsl_check_launch("conv_tc2");
 }
 
 template <int KS, int KBLK, int MT>
-int conv2_dispatch_nt(int nt, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, cudaStream_t st) {
+int conv2_dispatch_nt(int nt, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& o, const ConvV2Params& p,
+                      cudaStream_t st) {
   return with_dt(p.dt, [&](auto dt) {
     constexpr int DT = decltype(dt)::value;
     switch (nt) {
-      case 16:  return launch_conv2<KS, KBLK, 16, MT, DT>(a0, a1, b, p, st);
-      case 32:  return launch_conv2<KS, KBLK, 32, MT, DT>(a0, a1, b, p, st);
-      case 64:  if constexpr (MT <= 2) return launch_conv2<KS, KBLK, 64, MT, DT>(a0, a1, b, p, st); else break;
-      case 128: if constexpr (MT == 1) return launch_conv2<KS, KBLK, 128, MT, DT>(a0, a1, b, p, st); else break;
+      case 16:  return launch_conv2<KS, KBLK, 16, MT, DT>(a0, a1, b, o, p, st);
+      case 32:  return launch_conv2<KS, KBLK, 32, MT, DT>(a0, a1, b, o, p, st);
+      case 64:  if constexpr (MT <= 2) return launch_conv2<KS, KBLK, 64, MT, DT>(a0, a1, b, o, p, st); else break;
+      case 128: if constexpr (MT == 1) return launch_conv2<KS, KBLK, 128, MT, DT>(a0, a1, b, o, p, st); else break;
     }
     wsl_set_error("conv_tc2: unsupported N tile %d", nt);
     return -1;
@@ -1414,7 +1549,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_c
       }
     }
   }
-  if (p.out_mode == 0 && p.stat_partials) write_stat_partials<NT>(ls, lq, p.stat_partials, p.CoutP, 0);
+  __shared__ float s_stat[CONSUMER_WARPS][2][NT];
+  if (p.out_mode == 0 && p.stat_partials) write_stat_partials<NT>(ls, lq, p.stat_partials, p.CoutP, 0, s_stat);
 }
 
 template <int NT, int KBW, int KB, int DT>
@@ -1725,8 +1861,10 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
   int nt = CoutP >= 128 ? 128 : CoutP;
   while (nt > 16 && (CoutP % nt != 0 || (long long)T * CinP * nt * 2 > 148 * 1024 || mt * nt > 128)) nt >>= 1;
   WSL_REQUIRE(CoutP % nt == 0 && (long long)T * CinP * nt * 2 <= 152 * 1024, "wsl_conv_tc2: weights do not fit (Cin %d, NT %d)", CinP, nt);
+  // 16-bit outputs leave through TMA stores, whose global row pitch must be a multiple of 16 bytes
+  WSL_REQUIRE(out_mode != 0 || CoutStore % 8 == 0, "wsl_conv_tc2: 16-bit outputs need CoutStore %% 8 == 0 (got %d)", CoutStore);
   const int pad = ksize / 2;
-  CUtensorMap a0, a1, b;
+  CUtensorMap a0, a1, b, o;
   {
     long long d[4] = {C0, W, H, N};
     int bx[4] = {kblk, 8 + 2 * pad, 16 * mt + 2 * pad, 1};
@@ -1747,6 +1885,15 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
     int rc = get_map(wpk_bf16, 3, d, bx, kblk, &b, dtype);
     if (rc) return rc;
   }
+  if (out_mode == 0) {   // one box per 64 channels of the N tile (ConvV2Cfg::OUT_CH); TMA clips channels >= CoutStore
+    long long d[4] = {CoutStore, W, H, N};
+    const int och = nt < 64 ? nt : 64;
+    int bx[4] = {och, 8, 16 * mt, 1};
+    int rc = get_map(out, 4, d, bx, och, &o, dtype);
+    if (rc) return rc;
+  } else {
+    o = a0;
+  }
   ConvV2Params p;
   p.N = N; p.H = H; p.W = W; p.C0 = C0; p.C1 = C1; p.CoutP = CoutP; p.CoutStore = CoutStore;
   p.tiles_x = W / 8; p.tiles_y = H / (16 * mt); p.ntiles = N * p.tiles_x * p.tiles_y;
@@ -1754,7 +1901,7 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
   p.stat_partials = (out_mode == 0) ? stat_partials : nullptr;
 #define WSL_C2(KS_, KB_, MT_)                                                   \
   do {                                                                         \
-    int rc_ = conv2_dispatch_nt<KS_, KB_, MT_>(nt, a0, a1, b, p, stream);      \
+    int rc_ = conv2_dispatch_nt<KS_, KB_, MT_>(nt, a0, a1, b, o, p, stream);   \
     if (stat_rows_host) *stat_rows_host = g_conv2_last_rows;                   \
     return rc_;                                                                \
   } while (0)
