@@ -353,6 +353,36 @@ int wsl_uniform_fill(unsigned long long seed, const unsigned long long* seed_ptr
 int wsl_feat_noise_fwd(const void* f, int dtype, const float* z, int N, long long hwc, void* out, cudaStream_t stream);
 int wsl_feat_noise_bwd(const void* g, int dtype, const float* z, int N, long long hwc, void* acc, void* out, cudaStream_t stream);
 
+/* FCDiscriminator (networks/discriminator.py:58-101; trained by train_deep_adversarial_network_2D.py:107-178), disc_ops.cu.
+ * Every nn.Conv2d(k=4, stride=2, padding=1) runs as a 3x3 / stride-1 / pad-1 convolution (wsl_conv_tc, wsl_conv_direct, their
+ * dgrad packs and the 3x3 weight gradients) over the space-to-depth tensor T[n, Y, X, (a*2+b)*Cin + c] = x[n, 2Y+a, 2X+b, c] with a
+ * structured weight: 4x4 tap k of an axis sits at 3x3 tap (k+1)>>1, phase (k+1)&1; the other slots are zero.  dtype: 0 bf16, 1 fp32.
+ * wsl_disc_pack_input: map [N,C0,H,W] and feature [N,C1,H,W] fp32 (conv0 / conv1 inputs, :80-81) -> T [N,H/2,W/2,CP], CP >= 4(C0+C1),
+ * channels above 4(C0+C1) zero; wsl_disc_unpack_input_grad: its transpose (dmap / dfeature fp32 NCHW, either may be NULL). */
+int wsl_disc_pack_input(const float* map, int C0, const float* feature, int C1, int N, int H, int W, int CP, void* out, int dtype,
+                        cudaStream_t stream);
+int wsl_disc_unpack_input_grad(const void* dT, int dtype, int N, int H, int W, int CP, int C0, int C1, float* dmap, float* dfeature,
+                               cudaStream_t stream);
+/* LeakyReLU(slope) then Dropout2d (:86-87, :90-91; cs [N*C] in {0, 2} or NULL) fused with space-to-depth: y [N,H,W,C] -> T [N,H/2,W/2,4C];
+ * slope 1 and cs NULL is the plain repacking of conv0 + conv1, which has no activation (:83-85).  wsl_d2s_act_bwd: depth-to-space of
+ * dT times cs times LeakyReLU'(y) (y = the pre-activation; NULL allowed when slope == 1). */
+int wsl_s2d_act_fwd(const void* y, int dtype, int N, int H, int W, int C, float slope, const float* cs, void* out, cudaStream_t stream);
+int wsl_d2s_act_bwd(const void* dT, const void* y, int dtype, int N, int H, int W, int C, float slope, const float* cs, void* dy,
+                    cudaStream_t stream);
+/* 4x4 torch-layout weights w0 [Cout,C0,4,4] (+ w1 [Cout,C1,4,4], the second source of the first layer) -> structured 3x3 torch layout
+ * w3 [Cout,CP,3,3] for wsl_pack_conv_weights; bias_out (optional) = b0 (+ b1): conv0 + conv1 as one convolution.  wsl_disc_gather_wgrad:
+ * the 16 used slots of a 3x3 weight gradient dw3 [Cout,CP,3,3] -> dw0 (and dw1), written, not accumulated. */
+int wsl_disc_scatter_weights(const float* w0, const float* b0, int C0, const float* w1, const float* b1, int C1, int Cout, int CP,
+                             float* w3, float* bias_out, cudaStream_t stream);
+int wsl_disc_gather_wgrad(const float* dw3, int Cout, int CP, int C0, int C1, float* dw0, float* dw1, cudaStream_t stream);
+/* Head (:94-97): LeakyReLU(slope) -> AvgPool2d(7) of the 16x16 conv4 map y [N,16,16,C] (rows / columns 0..13) -> flatten in NCHW
+ * order (c*4 + i*2 + j) -> Linear(4C, 2): pooled [N,4C] (kept for the backward), logits [N,2] fp32.  wsl_disc_head_bwd: dy [N,16,16,C]
+ * (zero at rows / columns 14, 15) and the classifier gradients dwc [2,4C], dbc [2] (written; batch sums in a fixed order). */
+int wsl_disc_head_fwd(const void* y, int dtype, int N, int C, float slope, const float* wc, const float* bc, float* pooled, float* logits,
+                      cudaStream_t stream);
+int wsl_disc_head_bwd(const float* dlogits, const float* pooled, const void* y, int dtype, int N, int C, float slope, const float* wc,
+                      float* dwc, float* dbc, void* dy, cudaStream_t stream);
+
 /* layout helpers at the API boundary */
 int wsl_nchw_f32_to_nhwc(const float* src, int N, int Creal, int H, int W, int CP, void* dst, int dtype, float scale,
                          cudaStream_t stream);   /* dst = scale * src (the loss scale of the fp16 modes; 1 otherwise) */
