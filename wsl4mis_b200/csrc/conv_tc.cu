@@ -1376,7 +1376,9 @@ int conv2_dispatch_nt(int nt, const CUtensorMap& a0, const CUtensorMap& a1, cons
 // summed in registers by the thread that owns pixel c (a rolling pair of partial rows): no cross-thread traffic.
 //   warp 8: TMA producer (one [KBW ch x 130 px] box per input row and channel block; OOB zero fill = padding)
 //   warpgroup h: pixels 64h .. 64h+63 of the strip (MMA issue + epilogue).  The MMAs of input row i + 1 are issued before
-//   the output row that row i completes is stored, so the tensor core works through the stores.
+//   the output row that row i completes is stored, so the tensor core works through the stores.  16-bit output rows leave
+//   through TMA tensor stores from swizzled shared-memory slots; nothing in the epilogue branches on the thread index (such
+//   a branch while a group is in flight makes ptxas serialise every wgmma of the kernel, C7518).
 // Work item = (image, 128-pixel column strip, segment of RS output rows); persistent CTAs walk the items.
 // ================================================================================================
 constexpr int ROW_PX = 128;
@@ -1388,6 +1390,8 @@ __host__ __device__ constexpr int row_abytes(int kbw) { return ((130 * kbw * 2 +
 template <int NT, int KBW, int KB, int DT>
 __device__ __forceinline__ void row_mma(float (&acc)[3 * NT / 2], uint32_t a_row, uint32_t w_u) {
   constexpr int NG = 3 * NT, SWB = KBW * 2, ROW_ABYTES = row_abytes(KBW);
+  // the weights are loop-invariant: without this, ptxas hoists their descriptors out of the row loop and keeps them live
+  asm volatile("" : "+r"(w_u));
   wgmma_fence();
 #pragma unroll
   for (int kb = 0; kb < KB; ++kb) {
@@ -1403,16 +1407,32 @@ __device__ __forceinline__ void row_mma(float (&acc)[3 * NT / 2], uint32_t a_row
   wgmma_commit();
 }
 
-template <int NT, int KBW, int KB, int DT>
+// fp32 global store where `on` is set, as a predicated instruction (see tma_store_4d: no branch on the thread index while an
+// MMA group is in flight)
+__device__ __forceinline__ void st_f32_if(bool on, float* ptr, float v) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %0, 0;\n\t@p st.global.f32 [%1], %2;\n\t}" ::"r"((uint32_t)on), "l"(ptr), "f"(v)
+               : "memory");
+}
+
+// Staged 16-bit output rows: per consumer warpgroup ROW_OUT_SLOTS slots of 64 pixels x NT channels, each the swizzled box of
+// the output tensor map; consecutive stored rows alternate slots.
+constexpr int ROW_OUT_SLOTS = 2;
+__host__ __device__ constexpr int row_out_bytes(int nt) { return 2 * ROW_OUT_SLOTS * 64 * nt * 2; }
+
+// OM: output mode as a template parameter (0: 16-bit NHWC through TMA stores, 1: fp32 NCHW logits stored directly).
+template <int NT, int KBW, int KB, int DT, int OM>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
-                                                                  const __grid_constant__ CUtensorMap map_b, const ConvV2Params p,
+                                                                  const __grid_constant__ CUtensorMap map_b,
+                                                                  const __grid_constant__ CUtensorMap map_o, const ConvV2Params p,
                                                                   const int RS, const int w_bytes, const int STAGES) {
   constexpr int NG = 3 * NT;                              // accumulator columns of one input row (three filter rows)
   constexpr int SWB = KBW * 2, ROW_ABYTES = row_abytes(KBW);   // channel block = swizzle span: 32 B (16 ch) or 64 B (32 ch)
+  constexpr int SLOT_BYTES = 64 * NT * 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* w_smem = smem;                                 // [KB][dx][3*NT rows x SWB]
-  uint8_t* a_smem = smem + w_bytes;
+  uint8_t* o_smem = smem + w_bytes;                       // [warpgroup][slot] staged output rows (w_bytes is a multiple of 1024)
+  uint8_t* a_smem = o_smem + row_out_bytes(NT);
   uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + (size_t)STAGES * KB * ROW_ABYTES);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + STAGES;
@@ -1431,6 +1451,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_c
     fence_barrier_init();
     prefetch_tmap(&map_a0);
     prefetch_tmap(&map_b);
+    if (OM == 0) prefetch_tmap(&map_o);
   }
   __syncthreads();
 
@@ -1486,108 +1507,155 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_row_kernel(const __grid_c
 #pragma unroll
   for (int k = 0; k < NT / 4; ++k) ls[k] = lq[k] = 0.f;
   mbar_wait(w_bar, 0);
-  int s = 0, rel = 0;                   // next stage to consume / stage of the row whose MMA group is in flight
-  uint32_t sph = 0;
-  // One accumulator, one MMA group in flight: row i's group is folded into the partial rows as soon as it retires, then the
-  // group of the next row (of this item or the next one) is issued and runs while row i - 2 is rounded and stored.  A second
-  // accumulator would keep 3*NT/2 more floats live and spill under the 168-register limit of a 384-thread CTA.
-  float acc[NG / 2];
-  if (my_items > 0) {
-    mbar_wait(&a_full[s], sph);
-    row_mma<NT, KBW, KB, DT>(acc, a_u + (uint32_t)(s * KB * ROW_ABYTES), w_u);
-    if (++s == STAGES) { s = 0; sph ^= 1u; }
-  }
-  for (int it = 0; it < my_items; ++it) {
-    const int item = blockIdx.x + it * gridDim.x;
-    const int seg = item % segs, t1 = item / segs, strip = t1 % strips, n = t1 / strips;
-    const int y0 = seg * RS;
-    float pa[NT / 2], pb[NT / 2];       // partial output rows i-2 (dy 0 + 1 summed) and i-1 (dy 0)
+  // The CTA walks R = my_items * (RS + 2) input rows in the producer's order (row r sits in stage r % STAGES); every CTA has
+  // at least one item (the host keeps the grid <= items).
+  const int R = my_items * rows_in;
+  const bool store_thread = t == 0;     // issues (and waits for) the TMA stores of its warpgroup's 64 pixels
+  const bool stats = OM == 0 && p.stat_partials != nullptr;
+  uint8_t* o_wg = o_smem + h * ROW_OUT_SLOTS * SLOT_BYTES;
+  // staging offset of this thread's first pair: pixel frag_row, channel frag_col of its warpgroup's box
+  const uint32_t o_thr = out_stage_offset<NT, SLOT_BYTES>(frag_row(t), frag_col(t));
+  float pa[NT / 2], pb[NT / 2];         // partial output rows i-2 (dy 0 + 1 summed) and i-1 (dy 0)
+  float o[NT / 2];                      // output row i - 2 of the last folded row i, before rounding to the storage type
 #pragma unroll
-    for (int e = 0; e < NT / 2; ++e) pa[e] = pb[e] = 0.f;
-    for (int i = 0; i < rows_in; ++i) {
-      wgmma_wait<0>();
-      release_stage(&a_empty[rel]);
-      if (++rel == STAGES) rel = 0;
-      wgmma_fence_regs(acc);
-      // column 8*j + frag_col + b of E: filter row j / (NT/8), output channel 8*(j % (NT/8)) + frag_col + b
-      float o[NT / 2];                  // output row i - 2 (i >= 2), before rounding to the 16-bit type
+  for (int e = 0; e < NT / 2; ++e) pa[e] = pb[e] = 0.f;
+
+  int s_iss = 0, s_rel = 0;             // stage of the next row to issue / of the row whose group retires next
+  uint32_t ph_iss = 0;
+  auto issue = [&](float (&acc)[NG / 2]) {
+    mbar_wait(&a_full[s_iss], ph_iss);
+    row_mma<NT, KBW, KB, DT>(acc, a_u + (uint32_t)(s_iss * KB * ROW_ABYTES), w_u);
+    if (++s_iss == STAGES) { s_iss = 0; ph_iss ^= 1u; }
+  };
+  // acc holds the retired group of row r: free its stage and fold it into o and the partial rows.  The partial rows need no
+  // reset between items: what they hold at an item's first row reaches only the outputs of rows 0 and 1, which are not stored.
+  auto fold = [&](float (&acc)[NG / 2]) {
+    release_stage(&a_empty[s_rel]);
+    if (++s_rel == STAGES) s_rel = 0;
+    wgmma_fence_regs(acc);
+    // column 8*j + frag_col + b of E: filter row j / (NT/8), output channel 8*(j % (NT/8)) + frag_col + b
+#pragma unroll
+    for (int ii = 0; ii < 2; ++ii)
+#pragma unroll
+      for (int jj = 0; jj < NT / 8; ++jj)
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+          const int e = 4 * jj + 2 * ii + b;
+          o[e] = (pa[e] + acc[4 * (2 * NT / 8 + jj) + 2 * ii + b]) + s_bias[8 * jj + frag_col(t) + b];
+          pa[e] = pb[e] + acc[4 * (NT / 8 + jj) + 2 * ii + b];   // output row i - 1: + filter row 1
+          pb[e] = acc[4 * jj + 2 * ii + b];                       // output row i: filter row 0
+        }
+    wgmma_discard_regs(acc);
+  };
+  // output row i - 2 of the current item, complete once its row i >= 2 (the CTA's row r) is folded
+  int i = 0, n = 0, strip = 0, y0 = 0;
+  auto start_item = [&](int it) {
+    const int item = blockIdx.x + it * (int)gridDim.x;
+    const int seg = item % segs, t1 = item / segs;
+    strip = t1 % strips; n = t1 / strips; y0 = seg * RS;
+  };
+  auto store_row = [&](int r) {
+    if (i < 2) return;
+    const int gy = y0 + i - 2;
+    if constexpr (OM == 0) {
+      // Consecutive stored rows alternate slots (an item's rows 0 and 1 store nothing, which keeps the alternation), and the
+      // wait before the barrier of one row frees the slot the next row writes.
+      const uint32_t slot = (uint32_t)((r & 1) * SLOT_BYTES);
 #pragma unroll
       for (int ii = 0; ii < 2; ++ii)
+#pragma unroll
+        for (int jj = 0; jj < NT / 8; ++jj) {
+          const int e = 4 * jj + 2 * ii;
+          const uint32_t u = DT == 2 ? pack_f16(o[e], o[e + 1]) : pack_bf16(o[e], o[e + 1]);
+          if (stats) {                   // statistics of the values exactly as stored (rounded to the 16-bit type)
+            float2 v;
+            if (DT == 2) v = __half22float2(*reinterpret_cast<const __half2*>(&u));
+            else v = make_float2(bf16_lo(u), bf16_hi(u));
+            ls[2 * jj] += v.x;     lq[2 * jj] = fmaf(v.x, v.x, lq[2 * jj]);
+            ls[2 * jj + 1] += v.y; lq[2 * jj + 1] = fmaf(v.y, v.y, lq[2 * jj + 1]);
+          }
+          // pixel + 8 is NT * 16 bytes further on, which keeps the swizzle phase: channel group jj is an XOR of the base offset
+          *reinterpret_cast<uint32_t*>(o_wg + ((o_thr + slot + (uint32_t)(8 * ii * NT * 2)) ^ (uint32_t)(jj << 4))) = u;
+        }
+      fence_proxy_async();
+      bulk_wait_read_all(store_thread);  // the previous row's store has read the other slot
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + h) : "memory");
+      tma_store_4d(store_thread, &map_o, o_wg + slot, 0, strip * ROW_PX + 64 * h, gy, n);
+      bulk_commit(store_thread);
+    } else {
+      float* out = reinterpret_cast<float*>(p.out);
+#pragma unroll
+      for (int ii = 0; ii < 2; ++ii) {
+        const int gx = strip * ROW_PX + 64 * h + frag_row(t) + 8 * ii;
 #pragma unroll
         for (int jj = 0; jj < NT / 8; ++jj)
 #pragma unroll
           for (int b = 0; b < 2; ++b) {
-            const int e = 4 * jj + 2 * ii + b;
-            o[e] = (pa[e] + acc[4 * (2 * NT / 8 + jj) + 2 * ii + b]) + s_bias[8 * jj + frag_col(t) + b];
-            pa[e] = pb[e] + acc[4 * (NT / 8 + jj) + 2 * ii + b];   // output row i - 1: + filter row 1
-            pb[e] = acc[4 * jj + 2 * ii + b];                       // output row i: filter row 0
+            const int c = 8 * jj + frag_col(t) + b;
+            st_f32_if(c < p.CoutStore, out + (((long long)n * p.CoutStore + c) * p.H + gy) * p.W + gx, o[4 * jj + 2 * ii + b]);
           }
-      if (i + 1 < rows_in || it + 1 < my_items) {
-        mbar_wait(&a_full[s], sph);
-        row_mma<NT, KBW, KB, DT>(acc, a_u + (uint32_t)(s * KB * ROW_ABYTES), w_u);
-        if (++s == STAGES) { s = 0; sph ^= 1u; }
-      }
-      if (i >= 2) {                                   // output row i - 2 is complete
-        const int gy = y0 + i - 2;
-#pragma unroll
-        for (int ii = 0; ii < 2; ++ii) {
-          const int gx = strip * ROW_PX + 64 * h + frag_row(t) + 8 * ii;
-#pragma unroll
-          for (int jj = 0; jj < NT / 8; ++jj) {
-            const int c = 8 * jj + frag_col(t), e = 4 * jj + 2 * ii;
-            const float v0 = o[e], v1 = o[e + 1];
-            if (p.out_mode == 0 && p.stat_partials) {   // statistics of the values exactly as stored (rounded to the 16-bit type)
-              float2 r;
-              if (DT == 2) r = __half22float2(__floats2half2_rn(v0, v1));
-              else r = __bfloat1622float2(__floats2bfloat162_rn(v0, v1));
-              ls[2 * jj] += r.x;     lq[2 * jj] = fmaf(r.x, r.x, lq[2 * jj]);
-              ls[2 * jj + 1] += r.y; lq[2 * jj + 1] = fmaf(r.y, r.y, lq[2 * jj + 1]);
-            }
-            store_pair(p.out, p.out_mode == 0 ? 0 : 1, DT, p.CoutStore, p.H, p.W, n, gy, gx, c, v0, v1);
-          }
-        }
       }
     }
+  };
+
+  // One accumulator: row r is folded as soon as its group retires, then row r + 1's group is issued and runs while row r's
+  // output row is rounded, staged and stored.  A second accumulator would let row r + 1's group run under the fold as well,
+  // but ptxas then reports too few registers for the wgmma pipeline (C7511, at NT = 16 too) and serialises every MMA.  The
+  // last row is peeled: no MMA is issued on a path that joins one without a group in flight.
+  float acc[NG / 2];
+  issue(acc);
+  start_item(0);
+  for (int r = 0, it = 0;; ++r) {
+    wgmma_wait<0>();
+    fold(acc);
+    if (r + 1 == R) {
+      store_row(r);
+      break;
+    }
+    issue(acc);
+    store_row(r);
+    if (++i == rows_in) { i = 0; start_item(++it); }
   }
+  bulk_wait_all(store_thread);
   __shared__ float s_stat[CONSUMER_WARPS][2][NT];
-  if (p.out_mode == 0 && p.stat_partials) write_stat_partials<NT>(ls, lq, p.stat_partials, p.CoutP, 0, s_stat);
+  if (stats) write_stat_partials<NT>(ls, lq, p.stat_partials, p.CoutP, 0, s_stat);
 }
 
-template <int NT, int KBW, int KB, int DT>
-int launch_conv_row(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, int RS,
-                    cudaStream_t stream) {
+template <int NT, int KBW, int KB, int DT, int OM>
+int launch_conv_row(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& o, const ConvV2Params& p,
+                    int RS, cudaStream_t stream) {
   // Row buffers in flight: ~80 KB per SM cover the HBM latency.
   static const int st_env = [] { const char* e = getenv("WSL4MIS_ROW_STAGES"); return e ? atoi(e) : 0; }();
   const int STAGES = st_env ? st_env : (KB == 1 ? 12 : KB == 2 ? 8 : 6);
   const int w_bytes = ((KB * 9 * NT * KBW * 2 + 1023) / 1024) * 1024;
-  const int smem = w_bytes + STAGES * KB * row_abytes(KBW) + 1024 + 256;
+  const int smem = w_bytes + row_out_bytes(NT) + STAGES * KB * row_abytes(KBW) + 1024 + 256;
   if (smem > 220 * 1024) { wsl_set_error("conv_row: %d bytes of shared memory needed", smem); return -6; }
   static int attr_bytes = 0;
   if (smem > attr_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(conv_row_kernel<NT, KBW, KB, DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_row_kernel<NT, KBW, KB, DT, OM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { wsl_set_error("conv_row: cudaFuncSetAttribute(%d): %s", smem, cudaGetErrorString(e)); return -5; }
     attr_bytes = smem;
   }
   const int items = p.N * (p.W / ROW_PX) * (p.H / RS);
   int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_row_kernel<NT, KBW, KB, DT>, NUM_THREADS, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_row_kernel<NT, KBW, KB, DT, OM>, NUM_THREADS, smem);
   if (occ < 1) occ = 1;
   int gx = wsl_num_sms() * occ;
   if (gx > items) gx = items;
   g_conv2_last_rows = gx;
-  conv_row_kernel<NT, KBW, KB, DT><<<gx, NUM_THREADS, smem, stream>>>(a0, a1, b, p, RS, w_bytes, STAGES);
+  conv_row_kernel<NT, KBW, KB, DT, OM><<<gx, NUM_THREADS, smem, stream>>>(a0, a1, b, o, p, RS, w_bytes, STAGES);
   return wsl_check_launch("conv_row");
 }
 
 // KB = (C0 + C1) / KBW channel blocks: 1-4 at KBW = 16, 1-2 at KBW = 32 (the caller keeps C0 + C1 <= 64)
-template <int NT, int KBW, int DT>
-int conv_row_dispatch_kb(int KB, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const ConvV2Params& p, int RS,
-                         cudaStream_t stream) {
+template <int NT, int KBW, int DT, int OM>
+int conv_row_dispatch_kb(int KB, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& o,
+                         const ConvV2Params& p, int RS, cudaStream_t stream) {
   switch (KB) {
-    case 1: return launch_conv_row<NT, KBW, 1, DT>(a0, a1, b, p, RS, stream);
-    case 2: return launch_conv_row<NT, KBW, 2, DT>(a0, a1, b, p, RS, stream);
-    case 3: if constexpr (KBW == 16) return launch_conv_row<NT, KBW, 3, DT>(a0, a1, b, p, RS, stream); else break;
-    case 4: if constexpr (KBW == 16) return launch_conv_row<NT, KBW, 4, DT>(a0, a1, b, p, RS, stream); else break;
+    case 1: return launch_conv_row<NT, KBW, 1, DT, OM>(a0, a1, b, o, p, RS, stream);
+    case 2: return launch_conv_row<NT, KBW, 2, DT, OM>(a0, a1, b, o, p, RS, stream);
+    case 3: if constexpr (KBW == 16) return launch_conv_row<NT, KBW, 3, DT, OM>(a0, a1, b, o, p, RS, stream); else break;
+    case 4: if constexpr (KBW == 16) return launch_conv_row<NT, KBW, 4, DT, OM>(a0, a1, b, o, p, RS, stream); else break;
   }
   wsl_set_error("conv_row: unsupported channel block count %d", KB);
   return -1;
@@ -1805,6 +1873,8 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
   WSL_REQUIRE(out_mode == 0 || out_mode == 1, "wsl_conv_tc2: out_mode must be 0 (16-bit NHWC) or 1 (fp32 NCHW), got %d", out_mode);
   WSL_REQUIRE(C0 % 16 == 0 && C1 % 16 == 0 && C0 > 0, "wsl_conv_tc2: source channels must be multiples of 16 (got %d,%d)", C0, C1);
   WSL_REQUIRE(CoutP % 16 == 0, "wsl_conv_tc2: CoutP must be a multiple of 16");
+  // 16-bit outputs leave through TMA stores, whose global row pitch must be a multiple of 16 bytes
+  WSL_REQUIRE(out_mode != 0 || CoutStore % 8 == 0, "wsl_conv_tc2: 16-bit outputs need CoutStore %% 8 == 0 (got %d)", CoutStore);
   {   // narrow outputs at >= 128-pixel rows: the row kernel (filter rows in N) is 1.8-2.3x faster per pixel
     static const bool row_on = [] { const char* e = getenv("WSL4MIS_CONV_ROW"); return !(e && e[0] == '0'); }();
     static const bool wide_on = [] { const char* e = getenv("WSL4MIS_ROW_KBW32"); return !(e && e[0] == '0'); }();
@@ -1835,17 +1905,30 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
         int rc = get_map(wpk_bf16, 3, d, bx, kbw, &b, dtype);
         if (rc) return rc;
       }
+      CUtensorMap o;
+      if (out_mode == 0) {   // one box per warpgroup: CoutP channels x 64 pixels of one row; TMA clips channels >= CoutStore
+        long long d[4] = {CoutStore, W, H, N};
+        int bx[4] = {CoutP, 64, 1, 1};
+        int rc = get_map(out, 4, d, bx, CoutP, &o, dtype);
+        if (rc) return rc;
+      } else {
+        o = a0;
+      }
       ConvV2Params p;
       p.N = N; p.H = H; p.W = W; p.C0 = C0; p.C1 = C1; p.CoutP = CoutP; p.CoutStore = CoutStore;
       p.tiles_x = 0; p.tiles_y = 0; p.ntiles = 0;
       p.out_mode = out_mode; p.dt = dtype; p.bias = bias; p.out = out;
       p.stat_partials = (out_mode == 0) ? stat_partials : nullptr;
-      const int rc = with_dt(dtype, [&](auto dt) {
-        constexpr int DT = decltype(dt)::value;
-        return (CoutP == 16) ? conv_row_dispatch_kb<16, 16, DT>(KB, a0, a1, b, p, RS, stream)
-               : (kbw == 32) ? conv_row_dispatch_kb<32, 32, DT>(KB, a0, a1, b, p, RS, stream)
-                             : conv_row_dispatch_kb<32, 16, DT>(KB, a0, a1, b, p, RS, stream);
-      });
+      auto by_nt = [&](auto om) {
+        constexpr int OM = decltype(om)::value;
+        return with_dt(dtype, [&](auto dt) {
+          constexpr int DT = decltype(dt)::value;
+          return (CoutP == 16) ? conv_row_dispatch_kb<16, 16, DT, OM>(KB, a0, a1, b, o, p, RS, stream)
+                 : (kbw == 32) ? conv_row_dispatch_kb<32, 32, DT, OM>(KB, a0, a1, b, o, p, RS, stream)
+                               : conv_row_dispatch_kb<32, 16, DT, OM>(KB, a0, a1, b, o, p, RS, stream);
+        });
+      };
+      const int rc = out_mode == 0 ? by_nt(std::integral_constant<int, 0>{}) : by_nt(std::integral_constant<int, 1>{});
       if (stat_rows_host) *stat_rows_host = g_conv2_last_rows;
       return rc;
     }
@@ -1861,8 +1944,6 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
   int nt = CoutP >= 128 ? 128 : CoutP;
   while (nt > 16 && (CoutP % nt != 0 || (long long)T * CinP * nt * 2 > 148 * 1024 || mt * nt > 128)) nt >>= 1;
   WSL_REQUIRE(CoutP % nt == 0 && (long long)T * CinP * nt * 2 <= 152 * 1024, "wsl_conv_tc2: weights do not fit (Cin %d, NT %d)", CinP, nt);
-  // 16-bit outputs leave through TMA stores, whose global row pitch must be a multiple of 16 bytes
-  WSL_REQUIRE(out_mode != 0 || CoutStore % 8 == 0, "wsl_conv_tc2: 16-bit outputs need CoutStore %% 8 == 0 (got %d)", CoutStore);
   const int pad = ksize / 2;
   CUtensorMap a0, a1, b, o;
   {
