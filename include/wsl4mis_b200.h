@@ -377,11 +377,17 @@ int wsl_disc_scatter_weights(const float* w0, const float* b0, int C0, const flo
 int wsl_disc_gather_wgrad(const float* dw3, int Cout, int CP, int C0, int C1, float* dw0, float* dw1, cudaStream_t stream);
 /* Head (:94-97): LeakyReLU(slope) -> AvgPool2d(7) of the 16x16 conv4 map y [N,16,16,C] (rows / columns 0..13) -> flatten in NCHW
  * order (c*4 + i*2 + j) -> Linear(4C, 2): pooled [N,4C] (kept for the backward), logits [N,2] fp32.  wsl_disc_head_bwd: dy [N,16,16,C]
- * (zero at rows / columns 14, 15) and the classifier gradients dwc [2,4C], dbc [2] (written; batch sums in a fixed order). */
+ * (zero at rows / columns 14, 15) and the classifier gradients dwc [2,4C], dbc [2] (written; batch sums in a fixed order; both NULL: dy
+ * only, as in the DAN script's phase 1, whose discriminator gradients train_deep_adversarial_network_2D.py:176 discards). */
 int wsl_disc_head_fwd(const void* y, int dtype, int N, int C, float slope, const float* wc, const float* bc, float* pooled, float* logits,
                       cudaStream_t stream);
 int wsl_disc_head_bwd(const float* dlogits, const float* pooled, const void* y, int dtype, int N, int C, float slope, const float* wc,
                       float* dwc, float* dbc, void* dy, cudaStream_t stream);
+/* F.cross_entropy of the discriminator's logits [N,2] (train_deep_adversarial_network_2D.py:155-156 and :175): target 1 for the first
+ * n_ones rows, 0 for the rest (DAN_target, :135-137).  loss[0] = mean NLL (unweighted); dlogits [N,2] = (softmax - onehot) / N * weight,
+ * weight read from weight_ptr (device) when non-NULL, so a captured graph follows the ramped consistency weight (:151-152). */
+int wsl_disc_ce(const float* logits, int N, int n_ones, const float* weight_ptr, float weight, float* loss, float* dlogits,
+                cudaStream_t stream);
 
 /* layout helpers at the API boundary */
 int wsl_nchw_f32_to_nhwc(const float* src, int N, int Creal, int H, int W, int CP, void* dst, int dtype, float scale,
@@ -402,6 +408,14 @@ int wsl_pack_conv_weights_batched(const long long* table, int n_entries, long lo
  * grad_scale = 1/world_size turns the all-reduced gradient sum into DDP's mean. */
 int wsl_sgd_step(float* param, const float* grad, float* mom, long long n, const float* lr_ptr, float lr,
                  float momentum, float weight_decay, float grad_scale, cudaStream_t stream);
+
+/* optim.Adam(lr, betas, eps, weight_decay=0).step() over a flat fp32 buffer (train_deep_adversarial_network_2D.py:112-113,178), in
+ * the order and rounding of torch's multi-tensor path: exp_avg.lerp_(g, 1-beta1); exp_avg_sq.mul_(beta2).addcmul_(g, g, 1-beta2);
+ * denom = sqrt(exp_avg_sq) / bc2_sqrt + eps; param -= step_size * exp_avg / denom, with step_size = lr / (1 - beta1^t) and
+ * bc2_sqrt = sqrt(1 - beta2^t) for the step count t (after its increment).  The doubles are rounded to fp32 as torch rounds its
+ * Python scalars; scalars_ptr (device, {step_size, bc2_sqrt} in fp32) replaces the by-value pair so a captured graph follows t. */
+int wsl_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n, const float* scalars_ptr,
+                  double step_size, double bc2_sqrt, double beta1, double beta2, double eps, cudaStream_t stream);
 
 #ifdef __cplusplus
 }

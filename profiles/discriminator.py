@@ -6,8 +6,8 @@ Rows: phase 1 (B = 6, eval, gradients w.r.t. the map and the parameters), phase 
 train-mode batches of 32 and 64, each forward + backward, for this repository's discriminator in bf16 and fp32 mode and for the
 reference class (staged by oracle/stage_semi.py) on cuDNN at torch defaults and under bf16 autocast, on the same inputs.  Useful
 TFLOP/s counts the 4x4 / stride-2 convolutions' own work; the tensor cores execute 36/16 = 2.25x that (structured 3x3 weights).
-Then one full DAN iteration (both phases, this repository's UNet as the student) with each discriminator.  The card name and power
-limit are read in the same run."""
+Then one full DAN iteration (both phases, this repository's UNet as the student): the script's autograd body with each
+discriminator, and engine.DANStep eager and graph-captured, alternating.  The card name and power limit are read in the same run."""
 import argparse
 import os
 import subprocess
@@ -112,27 +112,37 @@ def main():
     dan_iteration(impls)
 
 
-def dan_iteration(impls, B=6, reps=10):
-    """train_deep_adversarial_network_2D.py:138-178 with this repository's UNet as the student, per discriminator"""
+def dan_iteration(impls, B=6, reps=10, rounds=3):
+    """train_deep_adversarial_network_2D.py:138-178 with this repository's UNet as the student: the script's autograd body with each
+    discriminator, and engine.DANStep (this repository's discriminator in bf16) eager and graph-captured.  The variants alternate
+    within each of `rounds` rounds; the table gives the median and the range over the rounds."""
     import wsl_oracle as O
+    from wsl4mis_b200.engine import DANStep
+    from wsl4mis_b200.networks.discriminator import FCDiscriminator
     from wsl4mis_b200.networks.unet import UNet
     from wsl4mis_b200.utils import losses
-    student = UNet(1, 4)
-    student.load_state_dict(O.synth_params(1, 4, ("decoder",), 7))
-    student = student.to(DEV)
+
+    def new_student():
+        s = UNet(1, 4)
+        s.load_state_dict(O.synth_params(1, 4, ("decoder",), 7))
+        return s.to(DEV)
+
+    student = new_student()
     opt = torch.optim.SGD(student.parameters(), lr=0.01, momentum=0.9, weight_decay=1e-4)
     xl, yl = O.synth_batch(B, 256, 256, seed=3, dense=True)
     xl, yl = xl.to(DEV), yl.to(DEV)
     xu = xl.flip(3).contiguous()
     dice = losses.DiceLoss(4)
     tgt = torch.tensor([1] * B + [0] * B, device=DEV)
-    print(f"\nfull DAN iteration (B = {B} labelled + {B} unlabelled, student UNet bf16, SGD + Adam):")
+    print(f"\nfull DAN iteration (B = {B} labelled + {B} unlabelled, student UNet bf16, SGD + Adam), {rounds} alternating rounds "
+          f"of {reps} iterations:")
+    variants = {}
     for name, (disc, ac) in impls.items():
         if name == "ours fp32":
             continue
         dopt = torch.optim.Adam(disc.parameters(), lr=1e-4, betas=(0.9, 0.99))
 
-        def it():
+        def it(disc=disc, ac=ac, dopt=dopt):
             student.train()
             disc.eval()
             ol, ou = student(xl), student(xu)
@@ -154,8 +164,23 @@ def dan_iteration(impls, B=6, reps=10):
             dopt.zero_grad()
             dl.backward()
             dopt.step()
-        ms = timed(it, reps)
-        print(f"  {name:20s} {ms:8.2f} ms / iteration  ({2 * B * 1e3 / ms:.0f} labelled + unlabelled images/s)")
+        variants["autograd, " + name] = it
+    steps = {}
+    for graph in (False, True):
+        d = FCDiscriminator(4)
+        d.load_state_dict(D.synth_params(101))
+        steps[graph] = DANStep(new_student(), d.to(DEV), graph=graph)
+        variants["DANStep " + ("graph" if graph else "eager")] = lambda st=steps[graph]: st(xl, yl, xu)
+    times = {k: [] for k in variants}
+    for r in range(rounds):
+        for name, fn in variants.items():
+            times[name].append(timed(fn, reps))
+    for name, ts in times.items():
+        ts = sorted(ts)
+        ms = ts[len(ts) // 2]
+        print(f"  {name:32s} {ms:8.2f} ms / iteration  (range {ts[0]:.2f}-{ts[-1]:.2f}; {2 * B * 1e3 / ms:.0f} labelled + unlabelled "
+              f"images/s)")
+    print(f"  DANStep launches per step: {steps[False].launches_per_step}")
 
 
 if __name__ == "__main__":

@@ -235,6 +235,25 @@ __global__ void __launch_bounds__(DTPB) head_bwd_param_kernel(const float* __res
   }
 }
 
+// 2-class cross entropy of logits [N][2] against targets 1 for rows < n_ones, 0 after (one warp, fixed summation order):
+// loss[0] = mean NLL; dl[n][c] = (softmax - onehot) * weight / N with weight = *weight_ptr when given
+__global__ void __launch_bounds__(32) disc_ce_kernel(const float* __restrict__ logits, int N, int n_ones, const float* weight_ptr,
+                                                     float weight, float* __restrict__ loss, float* __restrict__ dl) {
+  const float w = (weight_ptr ? *weight_ptr : weight) / (float)N;
+  float s = 0.f;
+  for (int n = threadIdx.x; n < N; n += 32) {
+    const float z0 = logits[2 * n], z1 = logits[2 * n + 1];
+    const float m = fmaxf(z0, z1);
+    const float e0 = expf(z0 - m), e1 = expf(z1 - m), se = e0 + e1;
+    const int t = n < n_ones ? 1 : 0;
+    s += logf(se) - ((t ? z1 : z0) - m);
+    dl[2 * n] = (e0 / se - (t ? 0.f : 1.f)) * w;
+    dl[2 * n + 1] = (e1 / se - (t ? 1.f : 0.f)) * w;
+  }
+  s = warp_sum(s);
+  if (threadIdx.x == 0) loss[0] = s / (float)N;
+}
+
 }  // namespace
 
 #define WSL_DISC_T(dtype, ...)                                   \
@@ -313,6 +332,15 @@ WSL_API int wsl_disc_head_bwd(const float* dlogits, const float* pooled, const v
   WSL_DISC_T(dtype, head_bwd_act_kernel<T><<<dgrid((long long)N * 256 * C), DTPB, 0, stream>>>(dlogits, (const T*)y, N, C, slope, wc, (T*)dy));
   int rc = wsl_check_launch("disc_head_bwd_act");
   if (rc) return rc;
+  WSL_REQUIRE((dwc == nullptr) == (dbc == nullptr), "wsl_disc_head_bwd: dwc and dbc are both given or both NULL");
+  if (dwc == nullptr) return 0;                    // map gradient only: no classifier gradients
   head_bwd_param_kernel<<<(8 * C + 2 + DTPB - 1) / DTPB, DTPB, 0, stream>>>(dlogits, pooled, N, 4 * C, dwc, dbc);
   return wsl_check_launch("disc_head_bwd_param");
+}
+
+WSL_API int wsl_disc_ce(const float* logits, int N, int n_ones, const float* weight_ptr, float weight, float* loss, float* dlogits,
+                        cudaStream_t stream) {
+  WSL_REQUIRE(N > 0 && n_ones >= 0 && n_ones <= N, "wsl_disc_ce: bad N=%d / n_ones=%d", N, n_ones);
+  disc_ce_kernel<<<1, 32, 0, stream>>>(logits, N, n_ones, weight_ptr, weight, loss, dlogits);
+  return wsl_check_launch("disc_ce");
 }

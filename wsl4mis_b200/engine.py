@@ -10,7 +10,8 @@
   pce_variance   train_weakly_supervised_pCE_Inter&Intra_Class_2D.py:112-125 (weight = consistency * sigmoid_rampup(it//150, 200))
   ce_dice        train_fully_supervised_2D.py:97-105 and train_weakly_supervised_pCE_random_walker_2D.py:97-104
                  (0.5 * (CE(ignore_index=4) + DiceLoss(softmax, label)) on dense or random-walker labels)
-(``S2LStep`` below adds Scribble2Label, train_s2l.py:119-157, and its ensemble refresh :214-243) as ONE launch sequence: executor forward -> fused loss head (softmax+pCE, regulariser, combined backward into
+(``S2LStep`` below adds Scribble2Label, train_s2l.py:119-157, and its ensemble refresh :214-243; ``DANStep`` the adversarial
+script, train_deep_adversarial_network_2D.py:126-184, with FCDiscriminator and a device Adam) as ONE launch sequence: executor forward -> fused loss head (softmax+pCE, regulariser, combined backward into
 dlogits) -> executor backward into a flat fp32 gradient bucket -> (NCCL all-reduce of that bucket when
 world_size > 1) -> fused SGD(momentum 0.9, wd 1e-4) over the flat parameter buffer with the poly LR read from
 device memory.  The whole sequence is CUDA-graph captured after the first call (graph=True).
@@ -684,3 +685,136 @@ class S2LStep(TrainStep):
             outs, _ = self.ex.forward(img, True, False, mk, None, bn_per_sample=True)
             max_hw = int(max(int(store.shapes[i, 0]) * int(store.shapes[i, 1]) for i in idx))
             call("wsl_s2l_refresh", outs[0], tab, B, size, max_hw, a, b, store.weight_live)
+
+
+class DANStep(_FlatSGDStep):
+    """Per-step body of train_deep_adversarial_network_2D.py:126-184 (adversarial semi-supervised training with FCDiscriminator).
+
+    Phase 1 (`_fwd_bwd`, :138-160; student in training mode, D in eval mode): training forwards of the labelled then the unlabelled
+    half (BatchNorm running statistics updated in that order), 0.5 * (Dice + CE) on the labelled half (CE without ignore_index), and
+    w(t) * CE(D(softmax(out_u), image_u), DAN_target[:B_u]) with w(t) = consistency * sigmoid_rampup(iter_num // 150, rampup).  That
+    term reaches the student through D's map gradient and the softmax Jacobian; D's own parameter gradients, which the script
+    discards (:176), are not computed.  Then SGD (momentum 0.9, weight decay 1e-4) at the poly learning rate.
+    Phase 2 (`_finish`, :162-178; student in eval mode, D in training mode with fresh Dropout2d masks): no-grad eval forwards of both
+    halves on the updated weights, D on cat(softmax_l, softmax_u) against [1]*B_l + [0]*B_u, and one Adam step of D
+    (`wsl_adam_step`, torch's multi-tensor arithmetic) over D's parameters, which live in one flat buffer (`dflat`).
+
+    D's operands are packed once per iteration, at the top of the step, into the executor's resident buffers; both phases read them
+    (D's weights change only in the Adam step at the end), and a `load_state_dict` between steps is picked up.  graph=True captures
+    the whole iteration as one CUDA graph after two eager warm-up steps; the ramp weight and Adam's t-dependent scalars are written
+    to `ramp_dev` before every step.  The modules' train() / eval() flags are not touched: each pass runs in the script's mode.
+    Test hooks: `model.dropout_masks` (phase 1) and `disc.channel_keep` (phase 2, [B_l + B_u, C] masks) as for the modules."""
+    aliases = ("parts",)
+    input_sets = 1
+
+    def __init__(self, model, disc, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0, disc_lr=1e-4,
+                 betas=(0.9, 0.99), graph=True, world_size=1):
+        if int(world_size) != 1:
+            raise NotImplementedError("DANStep runs on one GPU (world_size must be 1): the adversarial script has no multi-GPU form")
+        ex = model.executor
+        if len(getattr(ex, "dec", ())) != 1 or any(getattr(ex, "ds_heads", ())):
+            raise ValueError("DANStep needs a single-output segmentation network: the script takes torch.softmax(model(x), dim=1) "
+                             "(train_deep_adversarial_network_2D.py:143-144), which fails on a tuple of outputs")
+        from .utils import ramps
+        super().__init__(model, base_lr, max_iterations, 0.9, 1e-4, graph, 1, None)
+        self.ramps = ramps
+        self.segments = [[0, self.flat.numel()]]
+        self.n_trained = self.flat.numel()
+        self.consistency, self.consistency_rampup = float(consistency), float(consistency_rampup)
+        self.disc, self.dex = disc, disc.executor
+        if next(disc.parameters()).device != self.dev:
+            raise ValueError(f"DANStep: the discriminator is on {next(disc.parameters()).device}, the model on {self.dev}")
+        self.dflat, self.doffsets = _flatten(list(disc.parameters()), self.dev)
+        self.dgrad = torch.zeros_like(self.dflat)
+        self.exp_avg, self.exp_avg_sq = torch.zeros_like(self.dflat), torch.zeros_like(self.dflat)
+        self.adam_t = 0
+        self.disc_lr, self.betas, self.eps = float(disc_lr), (float(betas[0]), float(betas[1])), 1e-8
+        self.ramp_dev = torch.zeros(3, dtype=torch.float32, device=self.dev)   # {ramp weight, lr / (1 - b1^t), sqrt(1 - b2^t)}
+        self.parts = {}
+
+    def __call__(self, image_l, label_l, image_u):
+        """image_l / image_u: fp32 [B_l,1,256,256] / [B_u,1,256,256]; label_l: uint8 [B_l,256,256] dense.  Returns the phase-1 loss
+        (0-dim device tensor); `parts` holds loss_ce, loss_dice, consistency (the adversarial CE), weight and disc_loss."""
+        from .networks.discriminator import HW
+        for name, t in (("image_l", image_l), ("image_u", image_u)):
+            if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 4 and tuple(t.shape[1:]) == (self.disc.n_channel, HW, HW)):
+                raise ValueError(f"DANStep: {name} must be a CUDA fp32 [N, {self.disc.n_channel}, {HW}, {HW}] tensor (got "
+                                 f"{tuple(t.shape)} {t.dtype}); FCDiscriminator's kernels take the scripts' 256 x 256 patches")
+        if not (label_l.is_cuda and label_l.dtype == torch.uint8 and tuple(label_l.shape) == (image_l.shape[0], HW, HW)):
+            raise ValueError(f"DANStep: label_l must be a CUDA uint8 [{image_l.shape[0]}, {HW}, {HW}] tensor (got {tuple(label_l.shape)})")
+        if self.graph_enabled and image_u.shape[0] != image_l.shape[0]:
+            raise ValueError(f"DANStep(graph=True) needs B_u == B_l (got {image_u.shape[0]} and {image_l.shape[0]}): a captured graph has "
+                             f"fixed shapes; run the short last batch of an epoch with graph=False")
+        cw = self.consistency * self.ramps.sigmoid_rampup(self.iter_num // 150, self.consistency_rampup)     # :151-152
+        t = self.adam_t + 1
+        b1, b2 = self.betas
+        step_size, bc2_sqrt = self.disc_lr / (1 - b1 ** t), (1 - b2 ** t) ** 0.5          # as torch's Adam computes them (doubles)
+        self.ramp_dev.copy_(torch.tensor([cw, step_size, bc2_sqrt], dtype=torch.float32))
+        loss = self._run((image_l, label_l, image_u))
+        self.adam_t = t
+        self.parts = dict(self.parts, weight=cw)
+        return loss
+
+    def _softmax(self, logits, out, name):
+        N, C, H, W = logits.shape
+        call("wsl_softmax_pce_fwd", logits, None, out, N, C, H, W, 255, self.ex.buf("dan", name, (2,), torch.float32),
+             workspace("pce", self.dev))
+
+    def _fwd_bwd(self, image_l, label_l, image_u):
+        """phase 1 -> (loss, student gradient bucket)"""
+        ex, dex, dev = self.ex, self.dex, self.dev
+        B, _, H, W = image_l.shape
+        Bu, C = image_u.shape[0], 4
+        self._inputs = (image_l, image_u)
+        self._dpacks = dex.pack_resident(dev)
+        masks, ck = getattr(self.model, "dropout_masks", None), getattr(self.model, "channel_keep", None)
+        outs_l, slot_l = ex.forward(image_l.contiguous(), True, True, masks, ck)
+        outs_u, slot_u = ex.forward(image_u.contiguous(), True, True, masks, ck)
+        Bf = lambda name, shape, dt=torch.float32: ex.buf("dan", name, shape, dt)
+        # ---- supervised half: 0.5 * (Dice + CE) (:146-149), CE without ignore_index ----
+        probs, st = Bf("probs_l", (B, C, H, W)), Bf("stats_l", (2,))
+        call("wsl_softmax_pce_fwd", outs_l[0], label_l, probs, B, C, H, W, 255, st, workspace("pce", dev))
+        sums = Bf("dice", (13,))
+        call("wsl_pdice_fwd", probs, label_l, None, 1.0, B, C, H, W, sums, workspace("pdice", dev))
+        gp = Bf("gprobs_l", (B, C, H, W))
+        call("wsl_pdice_bwd", probs, label_l, None, 1.0, sums, B, C, H, W, 0.5, 0, gp)
+        dl_l = Bf("dl_l", (B, C, H, W))
+        call("wsl_head_bwd", probs, label_l, st, None, 0.5, gp, 1.0, B, C, H, W, 255, dl_l, None, ex.dt)
+        # ---- adversarial term (:151-157): D in eval mode on softmax(out_u); its gradient w.r.t. the map only ----
+        pu = Bf("probs_u", (Bu, C, H, W))
+        self._softmax(outs_u[0], pu, "stats_u")
+        logits, rec = dex.forward(pu, image_u.contiguous(), False, True, True, None, packs=self._dpacks)
+        adv, dlg = Bf("adv", (1,)), Bf("dlogits_u", (Bu, 2))
+        call("wsl_disc_ce", logits, Bu, min(B, Bu), self.ramp_dev[0:1], 0.0, adv, dlg)
+        dmap, _, _ = dex.backward(rec, dlg, True, False, param_grads=False)
+        dl_u = Bf("dl_u", (Bu, C, H, W))
+        call("wsl_head_bwd", pu, None, None, None, 0.0, dmap, 1.0, Bu, C, H, W, 255, dl_u, None, ex.dt)
+        loss = 0.5 * (sums[0] + st[0]) + self.ramp_dev[0] * adv[0]
+        self.parts = {"loss_ce": st[0], "loss_dice": sums[0], "consistency": adv[0]}
+        # ---- both backward passes through the shared student weights, accumulated in the flat bucket ----
+        ex.backward(slot_u, [dl_u], zero_grads=True)
+        g = ex.backward(slot_l, [dl_l], zero_grads=False)
+        return loss, g
+
+    def _finish(self, g, captured):
+        """student SGD (:158-160), then phase 2 (:162-178) and D's Adam step; host scalars come from ramp_dev in both modes"""
+        self._opt(g)
+        ex, dex, dev = self.ex, self.dex, self.dev
+        image_l, image_u = self._inputs
+        B, _, H, W = image_l.shape
+        Bu, C = image_u.shape[0], 4
+        N = B + Bu
+        Bf = lambda name, shape, dt=torch.float32: ex.buf("dan", name, shape, dt)
+        maps, imgs = Bf("maps", (N, C, H, W)), Bf("imgs", (N, 1, H, W))
+        self._softmax(ex.forward(image_l.contiguous(), False, False)[0][0], maps[:B], "stats_e")
+        self._softmax(ex.forward(image_u.contiguous(), False, False)[0][0], maps[B:], "stats_e")
+        imgs[:B].copy_(image_l)
+        imgs[B:].copy_(image_u)
+        logits, rec = dex.forward(maps, imgs, True, True, False, getattr(self.disc, "channel_keep", None), packs=self._dpacks)
+        dloss, dlg = Bf("disc_loss", (1,)), Bf("dlogits_d", (N, 2))
+        call("wsl_disc_ce", logits, N, B, None, 1.0, dloss, dlg)
+        dex.backward(rec, dlg, False, False, bucket=(self.dgrad, self.doffsets))
+        b1, b2 = self.betas
+        call("wsl_adam_step", self.dflat, self.dgrad, self.exp_avg, self.exp_avg_sq, self.dflat.numel(), self.ramp_dev[1:3], 0.0, 0.0,
+             b1, b2, self.eps)
+        self.parts["disc_loss"] = dloss[0]

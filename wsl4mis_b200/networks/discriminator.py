@@ -6,7 +6,8 @@ T[n, Y, X, (a*2+b)*Cin + c] = x[n, 2Y+a, 2X+b, c] with a structured weight (each
 zero), so the forward, data gradient and weight gradient are the existing 3x3 convolutions: the per-tap wgmma kernel in bf16 mode, the
 CUDA-core direct kernels in fp32 mode.  conv0 (map) and conv1 (feature) are one convolution over the packed pair with bias b0 + b1.
 The parameters are ordinary fp32 nn.Parameters (the DAN script updates them with torch.optim.Adam); the operands are repacked on every
-forward.  Only 256 x 256 inputs are accelerated: that is the scripts' patch size, and the only size of the reference's valid range
+forward of the module.  engine.DANStep instead packs once per iteration into the executor's resident buffers (pack_resident) and
+runs both of the script's discriminator passes on them.  Only 256 x 256 inputs are accelerated: that is the scripts' patch size, and the only size of the reference's valid range
 (conv4 output 14..20, fixed by Linear(ndf*32, 2)) whose half-resolution maps tile the 8 x 16 pixel tiles of the kernels."""
 import torch
 import torch.nn as nn
@@ -47,24 +48,38 @@ class _DiscExecutor:
         self._partials = None
 
     # ---- operands ----------------------------------------------------------------------------------------------------------------
-    def _pack(self, L, need_dgrad, dev):
-        """structured 3x3 weight -> forward pack (and the flipped / transposed data-gradient pack); bias (b0 + b1 for the first layer)"""
+    def _pack(self, L, need_dgrad, dev, out=None):
+        """structured 3x3 weight -> forward pack (and the flipped / transposed data-gradient pack); bias (b0 + b1 for the first layer).
+        out: (w3 scratch, forward pack, data-gradient pack, bias) buffers to write instead of new tensors"""
         c = L.convs
-        w3 = torch.empty(L.Cout * L.CP * 9, dtype=torch.float32, device=dev)
-        bias = torch.empty(L.Cout, dtype=torch.float32, device=dev)
+        n = 9 * L.Cout * L.CP
+        if out is not None:
+            w3, fwd, dgr, bias = out
+        else:
+            w3 = torch.empty(L.Cout * L.CP * 9, dtype=torch.float32, device=dev)
+            bias = torch.empty(L.Cout, dtype=torch.float32, device=dev)
+            pdt = torch.bfloat16 if self.dt == 0 else torch.float32
+            fwd = torch.empty(n, dtype=pdt, device=dev)
+            dgr = torch.empty(n, dtype=pdt, device=dev) if need_dgrad else None
         w1, b1 = (c[1].weight, c[1].bias) if len(c) > 1 else (None, None)
         call("wsl_disc_scatter_weights", c[0].weight.detach(), c[0].bias.detach(), L.cins[0], None if w1 is None else w1.detach(),
              None if b1 is None else b1.detach(), L.cins[1] if len(c) > 1 else 0, L.Cout, L.CP, w3, bias)
-        n = 9 * L.Cout * L.CP
         if self.dt == 0:
-            fwd = torch.empty(n, dtype=torch.bfloat16, device=dev)
-            dgr = torch.empty(n, dtype=torch.bfloat16, device=dev) if need_dgrad else None
             call("wsl_pack_conv_weights", w3, L.Cout, L.CP, 3, L.Cout, L.CP, 0, L.CP, None, None, fwd, dgr, 0)
         else:
-            fwd = torch.empty(n, dtype=torch.float32, device=dev)
-            dgr = torch.empty(n, dtype=torch.float32, device=dev) if need_dgrad else None
             call("wsl_pack_conv_weights", w3, L.Cout, L.CP, 3, L.Cout, L.CP, 0, L.CP, fwd, dgr, None, None, 0)
         return fwd, dgr, bias
+
+    def pack_resident(self, dev):
+        """Pack every layer's operands (forward and data-gradient packs, summed first-layer bias) into buffers this executor owns and
+        keeps, and return them for forward(..., packs=).  A caller that runs several passes on unchanged weights packs once for all
+        of them; the buffers keep their addresses, so a captured CUDA graph that packs and reads them stays valid."""
+        if getattr(self, "_resident", None) is None or self._resident[0][1].device != dev:
+            pdt = torch.bfloat16 if self.dt == 0 else torch.float32
+            self._resident = [(torch.empty(L.Cout * L.CP * 9, dtype=torch.float32, device=dev),
+                               torch.empty(9 * L.Cout * L.CP, dtype=pdt, device=dev), torch.empty(9 * L.Cout * L.CP, dtype=pdt, device=dev),
+                               torch.empty(L.Cout, dtype=torch.float32, device=dev)) for L in self.layers]
+        return [self._pack(L, True, dev, out=bufs) for L, bufs in zip(self.layers, self._resident)]
 
     def _conv(self, L, T, wpk, bias, N):
         h = L.h
@@ -84,8 +99,9 @@ class _DiscExecutor:
             call("wsl_conv_direct", dy, L.Cout, None, 0, 1, dpk, None, dT, 2, N, h, h, L.Cout, L.CP, L.CP, 3)
         return dT
 
-    def _wgrad(self, L, T, dy, N):
-        """-> (weight gradients of the layer's convs in torch layout, bias gradient)"""
+    def _wgrad(self, L, T, dy, N, out=None):
+        """-> (weight gradients of the layer's convs in torch layout, bias gradient); out: ([weight gradient per conv], bias gradient)
+        tensors to write instead of new ones"""
         h, dev = L.h, dy.device
         dw3 = torch.zeros(L.Cout * L.CP * 9, dtype=torch.float32, device=dev)
         if self.dt == 0:
@@ -94,22 +110,28 @@ class _DiscExecutor:
             call("wsl_wgrad_tc", T, L.CP, None, 0, dy, L.Cout, dw3, N, h, h, L.Cout, 3, 0, self._partials, self._partials.numel())
         else:
             call("wsl_wgrad_direct", T, L.CP, None, 0, 1, dy, 1, L.Cout, dw3, None, N, h, h, L.Cout, 3)
-        dws = [torch.empty_like(c.weight) for c in L.convs]
+        if out is not None:
+            dws, db = out
+            db.zero_()
+        else:
+            dws = [torch.empty_like(c.weight) for c in L.convs]
+            db = torch.zeros(L.Cout, dtype=torch.float32, device=dev)
         call("wsl_disc_gather_wgrad", dw3, L.Cout, L.CP, L.cins[0], L.cins[1] if len(L.cins) > 1 else 0, dws[0],
              dws[1] if len(dws) > 1 else None)
-        db = torch.zeros(L.Cout, dtype=torch.float32, device=dev)
         call("wsl_channel_sum", dy, self.dt, N * h * h, L.Cout, L.Cout, db, workspace("disc_csum", dev))
         return dws, db
 
     # ---- forward / backward ------------------------------------------------------------------------------------------------------
-    def forward(self, mp, feat, training, need_grad, need_input_grad, keep):
+    def forward(self, mp, feat, training, need_grad, need_input_grad, keep, packs=None):
+        """packs: what pack_resident() returned (the weights unchanged since); None packs the operands here"""
         N, dev = mp.shape[0], mp.device
         if self.seed_dev is None or self.seed_dev.device != dev:
             self.seed_dev = torch.full((1,), initial_rng_counter(), dtype=torch.int64, device=dev)
         if training:
             self.seed_dev.add_(1)
         L0 = self.layers[0]
-        packs = [self._pack(L, need_grad and (i > 0 or need_input_grad), dev) for i, L in enumerate(self.layers)]
+        if packs is None:
+            packs = [self._pack(L, need_grad and (i > 0 or need_input_grad), dev) for i, L in enumerate(self.layers)]
         T = torch.empty((N, HW // 2, HW // 2, L0.CP), dtype=self.act, device=dev)
         call("wsl_disc_pack_input", mp, L0.cins[0], feat, L0.cins[1], N, HW, HW, L0.CP, T, self.dt)
         Ts, ys, css = [T], [], []
@@ -143,21 +165,34 @@ class _DiscExecutor:
             call("wsl_chan_mask_gen", 6271 * i, self.seed_dev, N * C, DROP_P, cs)
         return cs
 
-    def backward(self, rec, dlogits, need_map, need_feat):
-        """-> (d map, d feature, [12 parameter gradients in model.parameters() order])"""
+    def backward(self, rec, dlogits, need_map, need_feat, param_grads=True, bucket=None):
+        """-> (d map, d feature, [12 parameter gradients in model.parameters() order]).
+        param_grads=False: no weight-gradient launches at all, only the input gradients (the list is None).
+        bucket: (flat fp32 buffer, {id(parameter): (offset, numel)}): the gradients are written into their slices of that buffer, and
+        the returned list holds views of it"""
         N, Ts, ys, css, packs = rec["N"], rec["Ts"], rec["ys"], rec["css"], rec["packs"]
         m, dev = self.model, dlogits.device
         C4 = self.layers[3].Cout
+        if bucket is not None:
+            flat, offsets = bucket
+            view = lambda p: flat[offsets[id(p)][0]: offsets[id(p)][0] + p.numel()].view_as(p)
         dy = torch.empty_like(ys[3])
-        dwc, dbc = torch.empty_like(m.classifier.weight), torch.empty_like(m.classifier.bias)
+        if not param_grads:
+            dwc = dbc = None
+        elif bucket is not None:
+            dwc, dbc = view(m.classifier.weight), view(m.classifier.bias)
+        else:
+            dwc, dbc = torch.empty_like(m.classifier.weight), torch.empty_like(m.classifier.bias)
         call("wsl_disc_head_bwd", dlogits.contiguous(), rec["pooled"], ys[3], self.dt, N, C4, SLOPE, m.classifier.weight.detach(), dwc, dbc, dy)
         grads = {}
         dmap = dfeat = None
         for i in range(3, -1, -1):
             L = self.layers[i]
-            dws, db = self._wgrad(L, Ts[i], dy, N)
-            for conv, dw in zip(L.convs, dws):
-                grads[id(conv.weight)], grads[id(conv.bias)] = dw, db
+            if param_grads:
+                out = None if bucket is None else ([view(c.weight) for c in L.convs], view(L.convs[0].bias))
+                dws, db = self._wgrad(L, Ts[i], dy, N, out)
+                for conv, dw in zip(L.convs, dws):
+                    grads[id(conv.weight)], grads[id(conv.bias)] = dw, db
             if i == 0 and not (need_map or need_feat):
                 break
             dT = self._dgrad(L, dy, packs[i][1], N)
@@ -173,8 +208,13 @@ class _DiscExecutor:
                 call("wsl_d2s_act_bwd", dT, None, self.dt, N, P.h, P.h, P.Cout, 1.0, None, dy)
             else:
                 call("wsl_d2s_act_bwd", dT, ys[i - 1], self.dt, N, P.h, P.h, P.Cout, SLOPE, css[i - 1], dy)
+        if not param_grads:
+            return dmap, dfeat, None
         grads[id(m.classifier.weight)], grads[id(m.classifier.bias)] = dwc, dbc
-        grads[id(m.conv1.bias)] = grads[id(m.conv0.bias)].clone()   # both biases feed the same sum
+        if bucket is not None:                                       # both biases feed the same sum
+            grads[id(m.conv1.bias)] = view(m.conv1.bias).copy_(grads[id(m.conv0.bias)])
+        else:
+            grads[id(m.conv1.bias)] = grads[id(m.conv0.bias)].clone()
         return dmap, dfeat, [grads[id(p)] for p in m.parameters()]
 
 
