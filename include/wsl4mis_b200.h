@@ -107,9 +107,12 @@ int wsl_class_variance_fwd(const float* image, const float* probs, int N, int C,
 int wsl_class_variance_bwd(const float* image, const float* probs, const float* stats, int N, int C, int H, int W,
                            float scale, int accumulate, float* gprobs, cudaStream_t stream);
 
-/* Uncertainty-aware mean-teacher consistency (train_uncertainty_aware_mean_teacher_2D.py:164-188): mean softmax of the T
- * stochastic teacher passes (mc_logits [T*B,4,H,W], script layout) -> entropy -> mask (u8 [B,H,W]) -> masked
- * softmax_mse_loss(student, teacher) (utils/losses.py:65-82) / (2*sum(mask)+1e-16).  out3 = {sum, count, loss}.
+/* Mean-teacher consistency between softmax(student) and softmax(teacher) (utils/losses.py:65-82, softmax_mse_loss), two modes:
+ * T >= 2 (even), uncertainty-aware (train_uncertainty_aware_mean_teacher_2D.py:164-188): mean softmax of the T stochastic
+ *   teacher passes (mc_logits [T*B,4,H,W], script layout) -> entropy -> mask (u8 [B,H,W]) -> masked squared distance summed
+ *   / (2*sum(mask)+1e-16); out3 = {sum, sum(mask), loss}.
+ * T = 0, unmasked (train_mean_teacher_2D.py:169-170): torch.mean of the squared distance over B*C*H*W; mc_logits and mask
+ *   may be NULL (the backward takes mask = NULL); out3 = {sum, B*C*H*W, loss}.
  * threshold / weight are read from device memory when the *_ptr is non-NULL (graph-capture friendly ramps). */
 int wsl_uamt_consistency_fwd(const float* student, const float* teacher, const float* mc_logits, int T, int B, int C, int H,
                              int W, const float* threshold_ptr, float threshold, uint8_t* mask, float* out3, float* ws,

@@ -520,7 +520,8 @@ __global__ void __launch_bounds__(TPB) tv_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------
-// K13: uncertainty-aware mean-teacher consistency (train_uncertainty_aware_mean_teacher_2D.py:164-188):
+// K13: mean-teacher consistency, in two modes.
+// T >= 2, uncertainty-aware (train_uncertainty_aware_mean_teacher_2D.py:164-188):
 //   p_bar  = mean_t softmax(mc_logits[t])                         (T stochastic teacher passes, :164-174)
 //   unc    = -sum_c p_bar log(p_bar + 1e-6)                       (:175-176)
 //   mask   = unc < threshold                                      (:184-186)
@@ -528,7 +529,9 @@ __global__ void __launch_bounds__(TPB) tv_kernel(
 //   loss   = sum(mask * dist) / (2 * sum(mask) + 1e-16)           (:187-188)
 // mc_logits is the [T*B,4,H,W] buffer the script fills with T/2 teacher calls on the twice-repeated batch:
 // row (2*B*i + r) holds pass t = 2i + r/B of sample r % B.
-// fwd: one pass, emits the mask (u8) and {sum masked dist, mask count, loss}; bwd: d loss/d student logits.
+// T = 0, unmasked (train_mean_teacher_2D.py:169-170): loss = mean over B*C*H*W of dist; mc_logits and mask are unused (NULL).
+// fwd: one pass, emits the mask (u8, T >= 2) and {sum of (masked) dist, count, loss} with count = sum(mask) (T >= 2) or
+// B*C*H*W (T = 0); bwd: d loss/d student logits, unmasked when mask is NULL.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void softmax4(const float (&x)[C4], float (&p)[C4]) {
   const float m = fmaxf(fmaxf(x[0], x[1]), fmaxf(x[2], x[3]));
@@ -549,24 +552,27 @@ __global__ void __launch_bounds__(TPB) uamt_consistency_fwd_kernel(
   const long long npix = (long long)B * HW;
   for (long long i = blockIdx.x * (long long)TPB + threadIdx.x; i < npix; i += (long long)gridDim.x * TPB) {
     const long long b = i / HW, o = i - b * HW;
-    float pbar[C4] = {0.f, 0.f, 0.f, 0.f};
-    for (int t = 0; t < T; ++t) {
-      const long long row = (long long)(t >> 1) * 2 * B + (long long)(t & 1) * B + b;
-      float x[C4], p[C4];
+    bool on = true;
+    if (T > 0) {
+      float pbar[C4] = {0.f, 0.f, 0.f, 0.f};
+      for (int t = 0; t < T; ++t) {
+        const long long row = (long long)(t >> 1) * 2 * B + (long long)(t & 1) * B + b;
+        float x[C4], p[C4];
 #pragma unroll
-      for (int c = 0; c < C4; ++c) x[c] = mc[(row * C4 + c) * HW + o];
-      softmax4(x, p);
+        for (int c = 0; c < C4; ++c) x[c] = mc[(row * C4 + c) * HW + o];
+        softmax4(x, p);
 #pragma unroll
-      for (int c = 0; c < C4; ++c) pbar[c] += p[c];
+        for (int c = 0; c < C4; ++c) pbar[c] += p[c];
+      }
+      float unc = 0.f;
+#pragma unroll
+      for (int c = 0; c < C4; ++c) {
+        const float q = pbar[c] / (float)T;
+        unc -= q * logf(q + 1e-6f);
+      }
+      on = unc < thr;
+      mask[i] = on ? 1 : 0;
     }
-    float unc = 0.f;
-#pragma unroll
-    for (int c = 0; c < C4; ++c) {
-      const float q = pbar[c] / (float)T;
-      unc -= q * logf(q + 1e-6f);
-    }
-    const bool on = unc < thr;
-    mask[i] = on ? 1 : 0;
     if (on) {
       float xs[C4], xt[C4], ps[C4], pt[C4];
 #pragma unroll
@@ -583,24 +589,27 @@ __global__ void __launch_bounds__(TPB) uamt_consistency_fwd_kernel(
   __shared__ double res[2];
   if (block_reduce_final<2, TPB>(acc, partials, ticket, res)) {
     if (threadIdx.x == 0) {
+      const double count = T > 0 ? res[1] : (double)npix * C4;
       out[0] = (float)res[0];
-      out[1] = (float)res[1];
-      out[2] = (float)(res[0] / (2.0 * res[1] + 1e-16));
+      out[1] = (float)count;
+      out[2] = (float)(T > 0 ? res[0] / (2.0 * count + 1e-16) : res[0] / count);
     }
   }
 }
 
-// d (w * loss) / d student logits = softmax-Jacobian applied to g_c = w * 2 * mask * (ps_c - pt_c) / (2*count + 1e-16)
+// d (w * loss) / d student logits = softmax-Jacobian applied to g_c = w * 2 * mask * (ps_c - pt_c) / (2*count + 1e-16), or,
+// with mask == NULL (T = 0), g_c = w * 2 * (ps_c - pt_c) / count
 __global__ void __launch_bounds__(TPB) uamt_consistency_bwd_kernel(
     const float* __restrict__ student, const float* __restrict__ teacher, const uint8_t* __restrict__ mask,
     const float* __restrict__ stats, const float* __restrict__ weight_ptr, float weight, int B, int HW,
     float* __restrict__ dlogits) {
-  const float w = (weight_ptr ? *weight_ptr : weight) * 2.f / (2.f * stats[1] + 1e-16f);
+  const float w = mask ? (weight_ptr ? *weight_ptr : weight) * 2.f / (2.f * stats[1] + 1e-16f)
+                       : (weight_ptr ? *weight_ptr : weight) * 2.f / stats[1];
   const long long npix = (long long)B * HW;
   for (long long i = blockIdx.x * (long long)TPB + threadIdx.x; i < npix; i += (long long)gridDim.x * TPB) {
     const long long b = i / HW, o = i - b * HW;
     float d[C4] = {0.f, 0.f, 0.f, 0.f};
-    if (mask[i]) {
+    if (!mask || mask[i]) {
       float xs[C4], xt[C4], ps[C4], pt[C4], g[C4];
 #pragma unroll
       for (int c = 0; c < C4; ++c) { xs[c] = student[(b * C4 + c) * HW + o]; xt[c] = teacher[(b * C4 + c) * HW + o]; }
@@ -1126,7 +1135,8 @@ WSL_API int wsl_tv_loss(const float* probs, int planes, int H, int W, float grad
 WSL_API int wsl_uamt_consistency_fwd(const float* student, const float* teacher, const float* mc_logits, int T, int B, int C,
                                      int H, int W, const float* threshold_ptr, float threshold, uint8_t* mask, float* out3,
                                      float* ws, cudaStream_t stream) {
-  WSL_REQUIRE(C == C4 && T >= 2 && T % 2 == 0, "wsl_uamt_consistency_fwd: C must be 4 and T even (got C=%d, T=%d)", C, T);
+  WSL_REQUIRE(C == C4 && T >= 0 && T % 2 == 0, "wsl_uamt_consistency_fwd: C must be 4 and T even (got C=%d, T=%d)", C, T);
+  WSL_REQUIRE(T == 0 || (mc_logits && mask), "wsl_uamt_consistency_fwd: T = %d needs mc_logits and mask", T);
   const long long npix = (long long)B * H * W;
   uamt_consistency_fwd_kernel<<<grid_for(npix, TPB), TPB, 0, stream>>>(student, teacher, mc_logits, T, B, H * W, threshold_ptr,
                                                                        threshold, mask, ws + 64, reinterpret_cast<unsigned*>(ws), out3);

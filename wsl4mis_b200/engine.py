@@ -11,7 +11,11 @@
   ce_dice        train_fully_supervised_2D.py:97-105 and train_weakly_supervised_pCE_random_walker_2D.py:97-104
                  (0.5 * (CE(ignore_index=4) + DiceLoss(softmax, label)) on dense or random-walker labels)
 (``S2LStep`` below adds Scribble2Label, train_s2l.py:119-157, and its ensemble refresh :214-243; ``DANStep`` the adversarial
-script, train_deep_adversarial_network_2D.py:126-184, with FCDiscriminator and a device Adam) as ONE launch sequence: executor forward -> fused loss head (softmax+pCE, regulariser, combined backward into
+script, train_deep_adversarial_network_2D.py:126-184, with FCDiscriminator and a device Adam; ``UAMTStep``, ``MeanTeacherStep``
+and ``EntropyMinStep`` the semi-supervised scripts train_uncertainty_aware_mean_teacher_2D.py, train_mean_teacher_2D.py and
+train_entropy_minimization_2D.py.  train_partially_fully_supervised.py:121-142 needs no class of its own: its body is
+0.5 * (CE + Dice) on the labelled batch, the unlabelled batch is loaded and never used, and on dense labels (no pixel is 4) the
+CE's ignore_index=4 of ``ce_dice`` ignores nothing, so ``TrainStep(model, 'ce_dice')`` fed the labelled batches runs it) as ONE launch sequence: executor forward -> fused loss head (softmax+pCE, regulariser, combined backward into
 dlogits) -> executor backward into a flat fp32 gradient bucket -> (NCCL all-reduce of that bucket when
 world_size > 1) -> fused SGD(momentum 0.9, wd 1e-4) over the flat parameter buffer with the poly LR read from
 device memory.  The whole sequence is CUDA-graph captured after the first call (graph=True).
@@ -63,7 +67,13 @@ class _FlatSGDStep:
     Graph mode keeps `input_sets` sets of static input buffers (``input_buffers(i)``).  With two, a caller can copy batch k+1
     from pinned host memory on a copy stream while the graph of batch k runs (bench.py's end-to-end leg does).  Tensors that are
     not one of those buffers are copied into set 0.  After two eager warm-up steps one graph is captured per input set, or per
-    host key for a step that passes one (such a step keeps a single input set), and replayed from then on."""
+    host key for a step that passes one (such a step keeps a single input set), and replayed from then on.
+
+    Graphs and static buffers are kept per batch shape as well: the semi-supervised scripts' loaders keep their short last
+    batches (no drop_last), so an epoch of ``zip(cycle(labelled), unlabelled)`` brings up to four shape combinations.  An input
+    set's buffers, and the graphs keyed by its index or host key alone, have the shape of the first batch that set saw; every
+    other shape gets its own buffers and graphs, keyed by (set index or host key, input shapes), after two eager warm-up steps at
+    that shape (they allocate the executor's buffers for it)."""
     aliases = ()            # attributes _fwd_bwd sets that alias graph memory: kept per graph and restored on every replay
     input_sets = 2
     nccl_in_graph = False   # world_size > 1: capture the all-reduce in the step graph instead of issuing it between two graphs
@@ -82,7 +92,8 @@ class _FlatSGDStep:
         self.mom = torch.zeros_like(self.flat)
         self.lr_dev = torch.full((1,), self.base_lr, dtype=torch.float32, device=self.dev)
         self.launches_per_step = 0
-        self._warm, self._graphs, self._static = 0, {}, [None] * self.input_sets
+        self._warm, self._graphs, self._static = {}, {}, [None] * self.input_sets
+        self._static_other = {}     # (input set, input shapes) -> buffers of the shapes an input set was not first called with
 
     def _opt(self, g):
         for off, n in self.segments:
@@ -111,26 +122,33 @@ class _FlatSGDStep:
 
     def _run(self, inputs, key=None, **kw):
         """One training step on `inputs` (the tensors `_fwd_bwd` reads; kw: its host arguments).  `key` names the host values a
-        captured graph bakes in (USTM's rot90 count); without one, graphs are keyed by input set.  Returns the loss (0-dim device
-        tensor)."""
+        captured graph bakes in (USTM's rot90 count); without one, graphs are keyed by input set, and by the input shapes when they
+        are not that set's first shapes.  Returns the loss (0-dim device tensor)."""
+        shapes = tuple(tuple(x.shape) for x in inputs)
         if self.graph_enabled:
             s = 0
             for i, st in enumerate(self._static):
                 if st is not None and st[0].data_ptr() == inputs[0].data_ptr():
                     s = i
             static = self.input_buffers(s, like=inputs)
+            home = tuple(tuple(b.shape) for b in static) == shapes
+            if not home:
+                if (s, shapes) not in self._static_other:
+                    self._static_other[(s, shapes)] = tuple(torch.empty_like(x) for x in inputs)
+                static = self._static_other[(s, shapes)]
             for buf, x in zip(static, inputs):
-                assert buf.shape == x.shape, "graph mode needs a fixed batch shape"
                 if buf.data_ptr() != x.data_ptr():
                     buf.copy_(x, non_blocking=True)
             inputs = static
-        if not self.graph_enabled or self._warm < 2:       # graph mode: the eager warm-up allocates every buffer / tensor map
+        if not self.graph_enabled or self._warm.get(shapes, 0) < 2:    # graph mode: the eager warm-up allocates every buffer / tensor map
             c0 = _lib.COUNTERS["launch_calls"]
             loss, _ = self._step(inputs, kw, False)
             self.launches_per_step = _lib.COUNTERS["launch_calls"] - c0
-            self._warm += 1
+            self._warm[shapes] = self._warm.get(shapes, 0) + 1
         else:
             k = s if key is None else key
+            if not home:
+                k = (k, shapes)
             if k not in self._graphs:
                 self._graphs[k] = self._capture(inputs, kw) + (tuple(getattr(self, a) for a in self.aliases),)
             g1, g2, gloss, gg, kept = self._graphs[k]
@@ -436,21 +454,22 @@ class UAMTStep(_FlatSGDStep):
         broadcast from rank 0 at construction; the teacher is never updated by the reference (SURVEY F8) and is broadcast once.
 
         graph=True: after two eager warm-up steps the whole body (two student forwards, 1 + T/2 teacher forwards, losses, two
-        backwards, SGD) is captured in ONE CUDA graph (world_size > 1: forward+backward | host-issued all-reduce | SGD, as
-        `TrainStep`) -- the eager step issues ~900 launches from Python and is host-bound.  The ramps of the script (consistency
-        weight :183, uncertainty threshold :186, poly LR :194) stay host arithmetic: they are written to a 2-float device buffer
-        before every replay and read by the kernels through their *_ptr arguments.  Needs a fixed batch shape and noises=None."""
+        backwards, SGD) is captured in ONE CUDA graph per batch shape (world_size > 1: forward+backward | host-issued all-reduce |
+        SGD, as `TrainStep`) -- the eager step issues ~900 launches from Python and is host-bound.  The ramps of the script
+        (consistency weight :183, uncertainty threshold :186, poly LR :194) stay host arithmetic: they are written to a 2-float
+        device buffer before every replay and read by the kernels through their *_ptr arguments.  Needs noises=None."""
         from .utils import ramps
         super().__init__(model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group)
         self.ramps = ramps
-        self.ema_model, self.ex_t = ema_model, ema_model.executor
+        self.ema_model = ema_model
+        self.ex_t = None if ema_model is None else ema_model.executor
         self.consistency, self.consistency_rampup = float(consistency), float(consistency_rampup)
         self.T = int(T)
         # the optimiser walks the prefix of the flat buffer in front of the first aux_decoder1 parameter
         first_aux = next(model.aux_decoder1.parameters()) if len(self.ex.dec) == 2 else None
         self.n_trained = self.flat.numel() if first_aux is None else self.offsets[id(first_aux)][0]
         self.segments = [[0, self.n_trained]]
-        if self.world_size > 1:
+        if self.world_size > 1 and ema_model is not None:
             for q in list(ema_model.parameters()) + list(ema_model.buffers()):
                 ddp.broadcast_flat(q.data, 0, self.pg)
         from .networks._engine import initial_rng_counter
@@ -471,6 +490,8 @@ class UAMTStep(_FlatSGDStep):
         B, _, H, W = img.shape
         tmasks, tck = getattr(self.ema_model, "dropout_masks", None), getattr(self.ema_model, "channel_keep", None)
         ema_out = ex_t.forward(self._noisy(img, 1, 0, None if noises is None else noises[0]), True, False, tmasks, tck)[0][0]
+        if not self.T:
+            return ema_out, None
         mc = self.ex.buf("teacher", "mc", (self.T * B, 4, H, W), torch.float32)
         for i in range(self.T // 2):
             tm2 = None if tmasks is None else {k: v.repeat(2, 1, 1, 1) for k, v in tmasks.items()}
@@ -491,7 +512,8 @@ class UAMTStep(_FlatSGDStep):
         """image_l/image_u: fp32 [B,1,H,W]; label_l: uint8 [B,H,W] dense.  noises (tests): list of 1 + T/2 tensors holding
         the already-clamped noise of :147-149 and :167-169.  Returns the loss (0-dim device tensor)."""
         self.model.train()
-        self.ema_model.train()
+        if self.ema_model is not None:
+            self.ema_model.train()
         thr, cw = self._ramps()
         assert noises is None or not self.graph_enabled, "graph mode draws the teacher noise on the device"
         loss = self._run((image_l, label_l, image_u), noises=noises)
@@ -501,37 +523,109 @@ class UAMTStep(_FlatSGDStep):
     def _fwd_bwd(self, image_l, label_l, image_u, noises=None):
         """forward passes, losses and both backward passes; returns (loss, flat gradient bucket)"""
         ex, dev = self.ex, self.dev
-        B, _, H, W = image_u.shape
-        C, T = 4, self.T
+        Bl, _, H, W = image_l.shape
+        C = 4
         self.seed_dev.add_(1)
         masks, ck = getattr(self.model, "dropout_masks", None), getattr(self.model, "channel_keep", None)
         outs_l, slot_l = ex.forward(image_l.contiguous(), True, True, masks, ck)
         outs_u, slot_u = ex.forward(image_u.contiguous(), True, True, masks, ck)
         out_l, out_u = outs_l[0], outs_u[0]
-        ema_out, mc = self._teacher(image_u, noises)
+        teacher = self._teacher(image_u, noises)
         Bf = lambda name, shape, dt=torch.float32: ex.buf("uamt", name, shape, dt)
         # ---- supervised half: 0.5 * (Dice + CE), CE without ignore_index (:127,:178-180) ----
-        probs, st = Bf("probs_l", (B, C, H, W)), Bf("stats_l", (2,))
-        call("wsl_softmax_pce_fwd", out_l, label_l, probs, B, C, H, W, 255, st, workspace("pce", dev))
+        probs, st = Bf("probs_l", (Bl, C, H, W)), Bf("stats_l", (2,))
+        call("wsl_softmax_pce_fwd", out_l, label_l, probs, Bl, C, H, W, 255, st, workspace("pce", dev))
         sums = Bf("dice", (13,))
-        call("wsl_pdice_fwd", probs, label_l, None, 1.0, B, C, H, W, sums, workspace("pdice", dev))
-        gp = Bf("gprobs_l", (B, C, H, W))
-        call("wsl_pdice_bwd", probs, label_l, None, 1.0, sums, B, C, H, W, 0.5, 0, gp)
-        dl_l = Bf("dl_l", (B, C, H, W))
-        call("wsl_head_bwd", probs, label_l, st, None, 0.5, gp, 1.0, B, C, H, W, 255, dl_l, None, self.ex.dt)
-        # ---- consistency half (:181-189) ----
-        # threshold (:186) and weight (:183) come from ramp_dev (written by _ramps() before the body / the graph replay)
-        mask, cst = Bf("mask", (B, H, W), torch.uint8), Bf("cons", (3,))
-        call("wsl_uamt_consistency_fwd", out_u, ema_out, mc, T, B, C, H, W, self.ramp_dev[0:1], 0.0, mask, cst, workspace("uamt", dev))
-        dl_u = Bf("dl_u", (B, C, H, W))
-        call("wsl_uamt_consistency_bwd", out_u, ema_out, mask, cst, self.ramp_dev[1:2], 0.0, B, C, H, W, dl_u)
-        loss = 0.5 * (sums[0] + st[0]) + self.ramp_dev[1] * cst[2]
-        self.parts = {"supervised": 0.5 * (sums[0] + st[0]), "consistency": cst[2], "mask": mask}
+        call("wsl_pdice_fwd", probs, label_l, None, 1.0, Bl, C, H, W, sums, workspace("pdice", dev))
+        gp = Bf("gprobs_l", (Bl, C, H, W))
+        call("wsl_pdice_bwd", probs, label_l, None, 1.0, sums, Bl, C, H, W, 0.5, 0, gp)
+        dl_l = Bf("dl_l", (Bl, C, H, W))
+        call("wsl_head_bwd", probs, label_l, st, None, 0.5, gp, 1.0, Bl, C, H, W, 255, dl_l, None, self.ex.dt)
+        # ---- unsupervised half (:181-189), weighted by ramp_dev[1] ----
+        cons, dl_u, mask = self._unsupervised(out_u, teacher, Bf)
+        loss = 0.5 * (sums[0] + st[0]) + self.ramp_dev[1] * cons
+        self.parts = {"supervised": 0.5 * (sums[0] + st[0]), "consistency": cons, "mask": mask}
         # ---- two backward passes through the shared student weights, gradients accumulated in the flat bucket ----
         nd = len(ex.dec)
         ex.backward(slot_u, [dl_u] + [None] * (nd - 1), zero_grads=True)
         g = ex.backward(slot_l, [dl_l] + [None] * (nd - 1), zero_grads=False)
         return loss, g
+
+    def _unsupervised(self, out_u, teacher, Bf):
+        """the consistency term -> (its value, a 0-dim device tensor; w * its logit gradient; the uncertainty mask or None).
+        Threshold (:186) and weight (:183) come from ramp_dev (written by _ramps() before the body / the graph replay)."""
+        ema_out, mc = teacher
+        B, C, H, W = out_u.shape
+        mask, cst = (Bf("mask", (B, H, W), torch.uint8) if self.T else None), Bf("cons", (3,))
+        call("wsl_uamt_consistency_fwd", out_u, ema_out, mc, self.T, B, C, H, W, self.ramp_dev[0:1], 0.0, mask, cst,
+             workspace("uamt", self.dev))
+        dl_u = Bf("dl_u", (B, C, H, W))
+        call("wsl_uamt_consistency_bwd", out_u, ema_out, mask, cst, self.ramp_dev[1:2], 0.0, B, C, H, W, dl_u)
+        return cst[2], dl_u, mask
+
+
+class MeanTeacherStep(UAMTStep):
+    """Per-step body of train_mean_teacher_2D.py:138-180 on the fused kernels: `UAMTStep` without the uncertainty estimate.
+
+    Student: training forwards with gradient on the labelled then the unlabelled batch (two BatchNorm batches, running statistics
+    updated in that order).  Teacher (`ema_model`): one training-mode no-grad forward on unlabelled + clamp(0.1 * randn, +-0.2)
+    (:147-149, :157-159).  Loss = 0.5 * (Dice + CE) on the labelled batch (dense labels, CE without ignore_index, :127) +
+    w(t) * torch.mean((softmax(student_u) - softmax(teacher))^2) (:169-170, the consistency kernels' T = 0 mode) with
+    w(t) = consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) (:73-75, :164-165); two backward passes into one
+    bucket, then SGD at the poly learning rate.  As written in the script, the teacher is never updated and never put in eval
+    mode (update_ema_variables is defined but not called, SURVEY F8).
+
+    graph=True: one CUDA graph per batch shape after two eager warm-up steps at that shape (see `_FlatSGDStep`); the ramp weight
+    is read from device memory.  world_size > 1: batch-sharded data parallel as `UAMTStep` (teacher broadcast once).  Two-head
+    models use main_seg on both sides (SURVEY F7)."""
+
+    def __init__(self, model, ema_model, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0,
+                 momentum=0.9, weight_decay=1e-4, world_size=1, process_group=None, graph=False, global_batch=False):
+        if global_batch:
+            raise NotImplementedError("global_batch semantics are not defined for the mean-teacher step (run it with per-rank normalisers)")
+        super().__init__(model, ema_model, base_lr=base_lr, max_iterations=max_iterations, consistency=consistency,
+                         consistency_rampup=consistency_rampup, momentum=momentum, weight_decay=weight_decay, T=0,
+                         process_group=process_group, world_size=world_size, graph=graph)
+
+    def _ramps(self):
+        """the consistency weight of :164-165 -> (None: no threshold, weight), also written to ramp_dev[1]"""
+        cw = self.consistency * self.ramps.sigmoid_rampup(self.iter_num // 300, self.consistency_rampup)
+        self.ramp_dev.copy_(torch.tensor([0.0, cw], dtype=torch.float32))
+        return None, cw
+
+
+class EntropyMinStep(UAMTStep):
+    """Per-step body of train_entropy_minimization_2D.py:121-150 on the fused kernels.
+
+    The student forwards and the supervised half of `MeanTeacherStep` (no teacher); the unsupervised term is
+    w(t) * losses.entropy_loss(softmax(student_u), C=4) (:141, utils/losses.py:30-36) with the same ramp
+    w(t) = consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) (:139).  graph=True and world_size > 1 as
+    `MeanTeacherStep`."""
+    _ramps = MeanTeacherStep._ramps
+
+    def __init__(self, model, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0, momentum=0.9,
+                 weight_decay=1e-4, world_size=1, process_group=None, graph=False, global_batch=False):
+        if global_batch:
+            raise NotImplementedError("global_batch semantics are not defined for the entropy-minimisation step (run it with per-rank normalisers)")
+        super().__init__(model, None, base_lr=base_lr, max_iterations=max_iterations, consistency=consistency,
+                         consistency_rampup=consistency_rampup, momentum=momentum, weight_decay=weight_decay, T=0,
+                         process_group=process_group, world_size=world_size, graph=graph)
+
+    def _teacher(self, img, noises):
+        return None
+
+    def _unsupervised(self, out_u, teacher, Bf):
+        B, C, H, W = out_u.shape
+        probs, ent = Bf("probs_u", (B, C, H, W)), Bf("ent", (1,))
+        call("wsl_softmax_pce_fwd", out_u, None, probs, B, C, H, W, 255, Bf("stats_u", (2,)), workspace("pce", self.dev))
+        call("wsl_entropy_fwd", probs, B, C, H, W, ent, workspace("ent", self.dev))
+        gp, dl_u = Bf("gprobs_u", (B, C, H, W)), Bf("dl_u", (B, C, H, W))
+        call("wsl_entropy_bwd", probs, B, C, H, W, 1.0, 0, gp)
+        # the ramp weight scales the probability gradient from device memory, so one captured graph serves every iteration
+        # (wsl_entropy_bwd takes its scale as a launch argument, and wsl_head_bwd's grad_out scales the CE term only)
+        gp.mul_(self.ramp_dev[1])
+        call("wsl_head_bwd", probs, None, None, None, 0.0, gp, 1.0, B, C, H, W, 255, dl_u, None, self.ex.dt)
+        return ent[0], dl_u, None
 
 
 class USTMStep(UAMTStep):
@@ -701,8 +795,8 @@ class DANStep(_FlatSGDStep):
 
     D's operands are packed once per iteration, at the top of the step, into the executor's resident buffers; both phases read them
     (D's weights change only in the Adam step at the end), and a `load_state_dict` between steps is picked up.  graph=True captures
-    the whole iteration as one CUDA graph after two eager warm-up steps; the ramp weight and Adam's t-dependent scalars are written
-    to `ramp_dev` before every step.  The modules' train() / eval() flags are not touched: each pass runs in the script's mode.
+    the whole iteration as one CUDA graph per batch shape after two eager warm-up steps at that shape: the first batch, a full one
+    with B_u == B_l, and after it an epoch's shorter last batches; the ramp weight and Adam's t-dependent scalars are written to `ramp_dev` before every step.  The modules' train() / eval() flags are not touched: each pass runs in the script's mode.
     Test hooks: `model.dropout_masks` (phase 1) and `disc.channel_keep` (phase 2, [B_l + B_u, C] masks) as for the modules."""
     aliases = ("parts",)
     input_sets = 1
@@ -742,9 +836,10 @@ class DANStep(_FlatSGDStep):
                                  f"{tuple(t.shape)} {t.dtype}); FCDiscriminator's kernels take the scripts' 256 x 256 patches")
         if not (label_l.is_cuda and label_l.dtype == torch.uint8 and tuple(label_l.shape) == (image_l.shape[0], HW, HW)):
             raise ValueError(f"DANStep: label_l must be a CUDA uint8 [{image_l.shape[0]}, {HW}, {HW}] tensor (got {tuple(label_l.shape)})")
-        if self.graph_enabled and image_u.shape[0] != image_l.shape[0]:
-            raise ValueError(f"DANStep(graph=True) needs B_u == B_l (got {image_u.shape[0]} and {image_l.shape[0]}): a captured graph has "
-                             f"fixed shapes; run the short last batch of an epoch with graph=False")
+        if self.graph_enabled and not self._warm and image_u.shape[0] != image_l.shape[0]:
+            raise ValueError(f"DANStep(graph=True) takes its first batch as the full batch and needs B_u == B_l there (got "
+                             f"{image_u.shape[0]} and {image_l.shape[0]}); an epoch's shorter last batches may follow, each captured "
+                             f"in its own graph")
         cw = self.consistency * self.ramps.sigmoid_rampup(self.iter_num // 150, self.consistency_rampup)     # :151-152
         t = self.adam_t + 1
         b1, b2 = self.betas
