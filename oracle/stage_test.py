@@ -1,0 +1,42 @@
+"""Stage the reference's UNMODIFIED test scripts (test_2D_fully.py, test_2D_fully_sps.py) under oracle/_ref/test/ (git-ignored build
+output that travels with the tree, like stage_semi.py's copies).  tests/test_test_2D_cpu.py compares their flags and fold split with
+wsl4mis_b200/test_2D.py.  A no-op where the reference is absent.
+
+    python oracle/stage_test.py           # __graft_entry__.build() calls it
+"""
+import hashlib
+import os
+import sys
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+REF = "/root/reference/code"
+OUT = os.path.join(HERE, "_ref", "test")
+FILES = ("test_2D_fully.py", "test_2D_fully_sps.py")
+
+
+def build():
+    """-> True when staged copies of both scripts exist afterwards"""
+    for rel in FILES:
+        src = os.path.join(REF, rel)
+        if os.path.exists(src):
+            os.makedirs(OUT, exist_ok=True)
+            data = open(src, "rb").read()
+            with open(os.path.join(OUT, rel), "wb") as f:
+                f.write(data)
+            with open(os.path.join(OUT, rel) + ".sha256", "w") as f:
+                f.write(hashlib.sha256(data).hexdigest())
+    return all(os.path.exists(os.path.join(OUT, r)) for r in FILES)
+
+
+def read(rel):
+    """source text of a staged script, checked against the digest written at staging time; None when nothing is staged"""
+    path = os.path.join(OUT, rel)
+    if not os.path.exists(path):
+        return None
+    data = open(path, "rb").read()
+    assert hashlib.sha256(data).hexdigest() == open(path + ".sha256").read().strip(), f"staged {rel} was modified"
+    return data.decode()
+
+
+if __name__ == "__main__":
+    sys.exit(0 if build() else 1)

@@ -243,6 +243,16 @@ def synthetic_acdc(n_patients=100, seed=2022, slices=(6, 11)):
     return cases
 
 
+def synthetic_spacing(patient, seed=2022):
+    """Voxel spacing (x, y, z) in mm of a `synthetic_acdc` case, in SimpleITK's GetSpacing order: slice distance from
+    {5, 6.5, 10}, each in-plane axis from {1.25, 1.37, 1.5625} (ACDC's range).  A stream of its own keyed by patient, so the
+    draws of `synthetic_acdc` stay as they are.  The two in-plane axes are drawn separately so that a mix-up of x and y shows."""
+    pid = int(str(patient).replace("patient", "").split("_")[0])
+    rs = np.random.RandomState([seed, pid])
+    inplane = (1.25, 1.37, 1.5625)
+    return float(inplane[rs.randint(3)]), float(inplane[rs.randint(3)]), float((5.0, 6.5, 10.0)[rs.randint(3)])
+
+
 class BaseDataSets(torch.utils.data.Dataset):
     """``BaseDataSets(base_dir, split, transform, fold, sup_type)`` as every WSS script constructs it
     (train_weakly_supervised_pCE_GatedCRFLoss_2D.py:75-80; the class the scripts need is the one in dataset_semi.py:17-125 --

@@ -56,9 +56,18 @@ def _device_mask(x, device=None):
     return m.to(device=dev, dtype=torch.uint8).contiguous()
 
 
-def surface_metrics(pred, gt, classes, voxelspacing=None):
+def surface_metrics_workspace_bytes(shape, classes):
+    """device bytes `surface_metrics` needs as workspace for volumes of `shape` ([S,H,W] or [H,W])"""
+    S, H, W = ((1,) + tuple(shape)) if len(shape) == 2 else tuple(shape)
+    nbytes = ctypes.c_longlong(0)
+    call("wsl_surface_metrics_workspace", len(shape), S, H, W, classes, ctypes.addressof(nbytes))
+    return nbytes.value
+
+
+def surface_metrics(pred, gt, classes, voxelspacing=None, workspace=None):
     """Counts, hd95 and asd of every class 1..classes-1 of two uint8 label volumes ([S,H,W] or [H,W], CUDA tensors) in one
-    kernel sequence.  Returns [SurfaceMetrics] indexed by class - 1."""
+    kernel sequence.  Returns [SurfaceMetrics] indexed by class - 1.  `workspace` (optional): a 256-byte aligned uint8 CUDA
+    tensor of at least `surface_metrics_workspace_bytes` bytes to use instead of a fresh allocation."""
     if pred.shape != gt.shape:
         raise ValueError(f"surface_metrics: shape mismatch {tuple(pred.shape)} vs {tuple(gt.shape)}")
     if pred.dim() not in (2, 3):
@@ -70,9 +79,13 @@ def surface_metrics(pred, gt, classes, voxelspacing=None):
     sp = _spacing(voxelspacing, ndim)
     sz, sy, sx = ((1.0,) + sp) if ndim == 2 else sp
     with torch.cuda.device(pred.device):
-        nbytes = ctypes.c_longlong(0)
-        call("wsl_surface_metrics_workspace", ndim, S, H, W, classes, ctypes.addressof(nbytes))
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=pred.device)
+        nbytes = surface_metrics_workspace_bytes(pred.shape, classes)
+        if workspace is None:
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=pred.device)
+        else:
+            if workspace.dtype != torch.uint8 or workspace.device != pred.device or workspace.numel() < nbytes:
+                raise ValueError(f"surface_metrics: workspace must be a uint8 tensor of >= {nbytes} bytes on {pred.device}")
+            ws = workspace
         out = torch.empty((classes - 1, 12), dtype=torch.float64, device=pred.device)
         call("wsl_surface_metrics", pred.contiguous(), gt.contiguous(), ndim, S, H, W, classes, sz, sy, sx, ws, out)
         o = out.cpu().numpy()
