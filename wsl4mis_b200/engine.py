@@ -26,6 +26,7 @@ torch.optim.SGD with ``grad is None``, is skipped by the optimiser.
 """
 from __future__ import annotations
 
+import math
 import os
 import random
 
@@ -34,6 +35,7 @@ import torch
 from . import ddp
 from . import _lib
 from ._lib import call, workspace
+from .utils import ramps
 
 VARIANTS = ("pce", "pce_gatedcrf", "pce_ms", "pce_tv", "dmpls", "pce_entropy", "pce_variance", "ce_dice")
 
@@ -59,6 +61,21 @@ def _captured(fn):
     return g, out
 
 
+def _ramp(consistency, iter_num, period, rampup):
+    """the scripts' consistency weight consistency * sigmoid_rampup(iter_num // period, rampup)"""
+    return consistency * ramps.sigmoid_rampup(iter_num // period, rampup)
+
+
+def _masks(model):
+    """the test hooks of `model` that fix its dropout: (dropout_masks, channel_keep), None where unset"""
+    return getattr(model, "dropout_masks", None), getattr(model, "channel_keep", None)
+
+
+def _aux_ids(model):
+    """ids of the aux decoder's parameters on a two-decoder model (unet_cct): steps that read main_seg only (SURVEY F7) skip them"""
+    return {id(q) for q in model.aux_decoder1.parameters()} if len(model.executor.dec) == 2 else set()
+
+
 class _FlatSGDStep:
     """What every step class shares: the flat fp32 master parameters, the fused SGD over the trained `segments` of that buffer
     with the poly LR read from device memory, and the driver `_run` that executes the subclass's
@@ -77,8 +94,12 @@ class _FlatSGDStep:
     aliases = ()            # attributes _fwd_bwd sets that alias graph memory: kept per graph and restored on every replay
     input_sets = 2
     nccl_in_graph = False   # world_size > 1: capture the all-reduce in the step graph instead of issuing it between two graphs
+    scratch = "step"        # executor buffer namespace of `_buf`
+    ramps = ramps
 
-    def __init__(self, model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group):
+    def __init__(self, model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group, skip):
+        """skip: ids of the parameters the step does not train.  Like torch.optim.SGD with grad=None, the fused optimiser leaves
+        them untouched: it walks the [offset, length] `segments` of the other parameters in the flat buffer."""
         self.model, self.ex = model, model.executor
         self.base_lr, self.max_iterations = float(base_lr), int(max_iterations)
         self.momentum, self.weight_decay = float(momentum), float(weight_decay)
@@ -90,10 +111,37 @@ class _FlatSGDStep:
         if self.world_size > 1:
             ddp.broadcast_flat(self.flat, 0, self.pg)     # identical replicas (DDP does the same at construction)
         self.mom = torch.zeros_like(self.flat)
+        self.segments = []
+        for p in self.ex.params:
+            if id(p) in skip:
+                continue
+            off, n = self.offsets[id(p)]
+            if self.segments and self.segments[-1][0] + self.segments[-1][1] == off:
+                self.segments[-1][1] += n
+            else:
+                self.segments.append([off, n])
+        self.n_trained = self.segments[-1][0] + self.segments[-1][1]     # prefix that holds every trained parameter (the all-reduce payload)
         self.lr_dev = torch.full((1,), self.base_lr, dtype=torch.float32, device=self.dev)
         self.launches_per_step = 0
         self._warm, self._graphs, self._static = {}, {}, [None] * self.input_sets
         self._static_other = {}     # (input set, input shapes) -> buffers of the shapes an input set was not first called with
+
+    def _buf(self, name, shape, dtype=torch.float32):
+        """the step's scratch tensor `name` of this shape (one per name, shape and dtype, kept by the executor)"""
+        return self.ex.buf(self.scratch, name, shape, dtype)
+
+    def _ce_dice(self, logits, label, ignore, ns, scale=1.0, d=None, d16=None):
+        """0.5 * (CE(ignore_index=`ignore`) + DiceLoss(softmax, label)) on dense labels -> (CE, Dice, loss), 0-dim device tensors;
+        `scale` times the logit gradient goes to `d` (fp32 NCHW) or `d16` (bf16 NHWC-16), scratch to buffer namespace `ns`.  The
+        Dice has no ignore mask (msum = NULL): a label-4 pixel is in no class but enters the Z sums, as one_hot(4) does."""
+        N, C, H, W = logits.shape
+        probs, gp = self.ex.buf(ns, "ce_dice.probs", (N, C, H, W), torch.float32), self.ex.buf(ns, "ce_dice.gprobs", (N, C, H, W), torch.float32)
+        st, sums = self.ex.buf(ns, "ce_dice.stats", (2,), torch.float32), self.ex.buf(ns, "ce_dice.sums", (13,), torch.float32)
+        call("wsl_softmax_pce_fwd", logits, label, probs, N, C, H, W, ignore, st, workspace("pce", self.dev))
+        call("wsl_pdice_fwd", probs, label, None, 1.0, N, C, H, W, sums, workspace("pdice", self.dev))
+        call("wsl_pdice_bwd", probs, label, None, 1.0, sums, N, C, H, W, 0.5, 0, gp)
+        call("wsl_head_bwd", probs, label, st, None, 0.5 * scale, gp, 1.0 * scale, N, C, H, W, ignore, d, d16, self.ex.dt)
+        return st[0], sums[0], 0.5 * (sums[0] + st[0])
 
     def _opt(self, g):
         for off, n in self.segments:
@@ -211,7 +259,13 @@ class TrainStep(_FlatSGDStep):
         and loss normalisers), which is what the weak-scaling benchmark runs.  The collectives are issued from the host inside the
         step, so this mode runs eagerly (no CUDA graph)."""
         assert variant in VARIANTS
-        super().__init__(model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group)
+        # Parameters that receive gradients in this step body: everything the executor runs except (a) the aux decoder when
+        # only main_seg enters the loss (SURVEY F7) and (b) deep-supervision heads (UNet_DS: the variants use output 0 only;
+        # out_conv_dp4 never runs at all).
+        skip = _aux_ids(model) if variant != "dmpls" else set()
+        skip.update(id(q) for nm, q in model.named_parameters() if "out_conv_dp" in nm)
+        skip.update(id(p) for p in model.executor.params if id(p) not in model.executor.used_param_ids)
+        super().__init__(model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group, skip)
         self.variant = variant
         self.global_batch = bool(global_batch) and self.world_size > 1
         if self.global_batch:
@@ -228,24 +282,6 @@ class TrainStep(_FlatSGDStep):
         self.n_heads_trained = 2 if (variant == "dmpls") else 1
         if variant == "dmpls":
             assert self.two_heads, "dmpls needs a two-head model (unet_cct)"
-        # Parameters that receive gradients in this step body: everything the executor runs except (a) the aux decoder when
-        # only main_seg enters the loss (SURVEY F7) and (b) deep-supervision heads (UNet_DS: the variants use output 0 only;
-        # out_conv_dp4 never runs at all).  Like torch.optim.SGD with grad=None, the fused optimiser leaves those untouched:
-        # it walks the contiguous segments of trained parameters in the flat buffer.
-        skip = set()
-        if self.two_heads and self.n_heads_trained == 1:
-            skip.update(id(q) for q in self.model.aux_decoder1.parameters())
-        skip.update(id(q) for nm, q in model.named_parameters() if "out_conv_dp" in nm)
-        self.segments = []
-        for p in self.ex.params:
-            if id(p) in skip or id(p) not in self.ex.used_param_ids:
-                continue
-            off_p, n_p = self.offsets[id(p)]
-            if self.segments and self.segments[-1][0] + self.segments[-1][1] == off_p:
-                self.segments[-1][1] += n_p
-            else:
-                self.segments.append([off_p, n_p])
-        self.n_trained = self.segments[-1][0] + self.segments[-1][1]     # prefix that holds every trained parameter (the all-reduce payload)
         # the encoder's parameters come first in parameters(): [0, enc_end) is final only at the very end of backward(), the
         # decoder slice [enc_end, n_trained) ~2 ms earlier -- its all-reduce is issued from inside backward() on a side stream
         self.enc_end = sum(q.numel() for q in model.encoder.parameters())
@@ -293,6 +329,11 @@ class TrainStep(_FlatSGDStep):
             raise NotImplementedError(f"global_batch semantics are not defined here for '{v}' (batch-slice TV / per-sample variance ramps)")
         if self.global_batch and v == "ce_dice":
             raise NotImplementedError("global_batch semantics are not defined here for 'ce_dice' (run it with per-rank normalisers)")
+        if v == "ce_dice":
+            d, d16, dl[0] = self._dlogits(ex, slot, "dl0", N, C, H, W)
+            ce, dice, loss = self._ce_dice(logits_list[0], label, 4, slot, S, d, d16)
+            self.loss_parts = {"ce": ce, "dice": dice}
+            return loss, dl
         heads = range(self.n_heads_trained)
         probs, stats = [], []
         for h in heads:
@@ -343,8 +384,7 @@ class TrainStep(_FlatSGDStep):
             loss = ce + 0.1 * out[0]
             dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, 1.0 * S * G, slot)
         elif v == "pce_variance":
-            from .utils import ramps
-            w = self.consistency * ramps.sigmoid_rampup(self.iter_num // 150, self.consistency_rampup)
+            w = _ramp(self.consistency, self.iter_num, 150, self.consistency_rampup)
             gp = B("gprobs0", (N, C, H, W))
             out = B("var", (3,))
             st = B("varstats", (N * C * 2 + N * 2,))
@@ -354,16 +394,6 @@ class TrainStep(_FlatSGDStep):
             self.cw_dev.fill_(w)
             loss = ce + self.cw_dev[0] * out[0]
             dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, float(w) * S, slot)
-        elif v == "ce_dice":
-            # DiceLoss(4)(softmax, label) has no ignore mask and no F14 weighting: pDLoss kernels with msum = NULL, mconst = 1
-            # (a label-4 pixel is in no class but its probabilities still enter the Z sums, as one_hot(4) does in the reference)
-            sums = B("dice0", (13,))
-            call("wsl_pdice_fwd", probs[0], label, None, 1.0, N, C, H, W, sums, workspace("pdice", dev))
-            gp = B("gprobs0", (N, C, H, W))
-            call("wsl_pdice_bwd", probs[0], label, None, 1.0, sums, N, C, H, W, 0.5, 0, gp)
-            loss = 0.5 * (ce + sums[0])
-            dl[0] = self._head_bwd(0, probs, stats, label, 0.5 * S, gp, 1.0 * S, slot)
-            self.loss_parts = {"ce": ce, "dice": sums[0]}
         else:  # dmpls
             pseudo = B("pseudo", (N, H, W), torch.uint8)
             call("wsl_mix_argmax", probs[0], probs[1], 0.0, 0.0, self.beta_dev, N, C, H, W, pseudo)   # beta from device memory
@@ -389,8 +419,7 @@ class TrainStep(_FlatSGDStep):
         # single-head scripts on the two-head model never read the aux output: let its forward keep running on the
         # side stream underneath the loss head and the main backward (joined at the end of the backward)
         defer = self.two_heads and self.n_heads_trained == 1
-        outs, slot = ex.forward(image, True, True, getattr(self.model, "dropout_masks", None),
-                                getattr(self.model, "channel_keep", None), defer_join=defer)
+        outs, slot = ex.forward(image, True, True, *_masks(self.model), defer_join=defer)
         loss, dl = self._head(outs, image, label, slot)
         ex.on_decoders_done = self._allreduce_decoders if self.overlap_comm else None
         try:
@@ -436,148 +465,156 @@ class TrainStep(_FlatSGDStep):
         return self._outs
 
 
-class UAMTStep(_FlatSGDStep):
-    """Per-step body of train_uncertainty_aware_mean_teacher_2D.py:138-197 (BASELINE config 5) on the fused kernels.
+class _NoisyTeacher:
+    """The never-updated teacher of the UAMT, MT and USTM steps (SURVEY F8): no-grad training-mode passes on noisy inputs, and the
+    softmax-MSE consistency against them (K13 kernels), masked by the uncertainty of T stochastic passes (T = 0: unmasked)."""
 
-    Batch = labelled half + unlabelled half.  Student: two training forwards with gradient (labelled, unlabelled);
-    teacher (`ema_model`, never updated and never put in eval mode by the reference, SURVEY F8): one no-grad forward on the
-    noisy unlabelled inputs and T/2 = 4 no-grad forwards on the twice-repeated noisy batch (T = 8 stochastic passes).
-    Loss = 0.5*(Dice + CE) on the labelled half + w(t) * uncertainty-masked softmax-MSE consistency (K13 kernels).
-    Two-head models (unet_cct) use main_seg on both sides (SURVEY F7)."""
-    aliases = ("parts",)
-    input_sets = 1          # USTM keys its graphs by the rot90 count alone
-
-    def __init__(self, model, ema_model, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0,
-                 momentum=0.9, weight_decay=1e-4, T=8, process_group=None, world_size=1, graph=False):
-        """world_size > 1: batch-sharded data parallel -- every rank runs the step on its shard, the flat gradient bucket is
-        all-reduced (sum) over NCCL and the fused SGD applies the 1/world mean, as `TrainStep` does.  The student replicas are
-        broadcast from rank 0 at construction; the teacher is never updated by the reference (SURVEY F8) and is broadcast once.
-
-        graph=True: after two eager warm-up steps the whole body (two student forwards, 1 + T/2 teacher forwards, losses, two
-        backwards, SGD) is captured in ONE CUDA graph per batch shape (world_size > 1: forward+backward | host-issued all-reduce |
-        SGD, as `TrainStep`) -- the eager step issues ~900 launches from Python and is host-bound.  The ramps of the script
-        (consistency weight :183, uncertainty threshold :186, poly LR :194) stay host arithmetic: they are written to a 2-float
-        device buffer before every replay and read by the kernels through their *_ptr arguments.  Needs noises=None."""
-        from .utils import ramps
-        super().__init__(model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group)
-        self.ramps = ramps
-        self.ema_model = ema_model
-        self.ex_t = None if ema_model is None else ema_model.executor
-        self.consistency, self.consistency_rampup = float(consistency), float(consistency_rampup)
-        self.T = int(T)
-        # the optimiser walks the prefix of the flat buffer in front of the first aux_decoder1 parameter
-        first_aux = next(model.aux_decoder1.parameters()) if len(self.ex.dec) == 2 else None
-        self.n_trained = self.flat.numel() if first_aux is None else self.offsets[id(first_aux)][0]
-        self.segments = [[0, self.n_trained]]
-        if self.world_size > 1 and ema_model is not None:
-            for q in list(ema_model.parameters()) + list(ema_model.buffers()):
-                ddp.broadcast_flat(q.data, 0, self.pg)
+    def __init__(self, model, T, dev, world_size, pg):
+        self.model, self.ex, self.T, self.dev = model, model.executor, int(T), dev
+        if world_size > 1:          # replicas start identical; the teacher is broadcast once
+            for q in list(model.parameters()) + list(model.buffers()):
+                ddp.broadcast_flat(q.data, 0, pg)
         from .networks._engine import initial_rng_counter
-        self.seed_dev = torch.full((1,), initial_rng_counter() ^ 0x5A5A5A5A, dtype=torch.int64, device=self.dev)
-        self.ramp_dev = torch.zeros(2, dtype=torch.float32, device=self.dev)       # {uncertainty threshold, consistency weight}
+        self.seed_dev = torch.full((1,), initial_rng_counter() ^ 0x5A5A5A5A, dtype=torch.int64, device=dev)
 
     def _noisy(self, x, reps, salt, given):
+        """x repeated `reps` times + clamp(0.1 * randn, +-0.2); given (tests): that noise"""
         if given is not None:
             return (x.repeat(reps, 1, 1, 1) + given).contiguous()
         out = torch.empty((x.shape[0] * reps,) + tuple(x.shape[1:]), dtype=torch.float32, device=self.dev)
         call("wsl_add_clamped_noise", x, x.numel(), reps, 0.1, 0.2, 0xA5A5 + salt, self.seed_dev, out)
         return out
 
-    def _teacher(self, img, noises):
-        """the teacher's no-grad passes on noisy copies of img: one at batch B -> ema_out, then T/2 on the twice-repeated batch
-        whose logits fill mc [T*B, C, H, W] in order.  noises (tests): the 1 + T/2 noise tensors; None draws them on the device"""
-        ex_t = self.ex_t
+    def __call__(self, img, noises):
+        """the passes on noisy copies of img: one at batch B -> ema_out, then T/2 on the twice-repeated batch whose logits fill
+        mc [T*B, C, H, W] in order (None when T = 0).  noises (tests): the 1 + T/2 noise tensors; None draws them on the device"""
+        self.seed_dev.add_(1)
         B, _, H, W = img.shape
-        tmasks, tck = getattr(self.ema_model, "dropout_masks", None), getattr(self.ema_model, "channel_keep", None)
-        ema_out = ex_t.forward(self._noisy(img, 1, 0, None if noises is None else noises[0]), True, False, tmasks, tck)[0][0]
+        tmasks, tck = _masks(self.model)
+        ema_out = self.ex.forward(self._noisy(img, 1, 0, None if noises is None else noises[0]), True, False, tmasks, tck)[0][0]
         if not self.T:
             return ema_out, None
-        mc = self.ex.buf("teacher", "mc", (self.T * B, 4, H, W), torch.float32)
+        mc = self.ex.buf("teacher", "mc", (self.T * B, self.ex.n_class, H, W), torch.float32)
         for i in range(self.T // 2):
             tm2 = None if tmasks is None else {k: v.repeat(2, 1, 1, 1) for k, v in tmasks.items()}
             tck2 = None if tck is None else [c.repeat(2, 1) for c in tck]
-            lg = ex_t.forward(self._noisy(img, 2, 1 + i, None if noises is None else noises[1 + i]), True, False, tm2, tck2)[0][0]
+            lg = self.ex.forward(self._noisy(img, 2, 1 + i, None if noises is None else noises[1 + i]), True, False, tm2, tck2)[0][0]
             mc[2 * B * i: 2 * B * (i + 1)].copy_(lg)
         return ema_out, mc
 
-    def _ramps(self):
-        """host arithmetic of :183 and :186 for the current iteration -> (threshold, weight), also written to ramp_dev"""
-        import math
-        cw = self.consistency * self.ramps.sigmoid_rampup(self.iter_num // 300, self.consistency_rampup)
-        thr = (0.75 + 0.25 * self.ramps.sigmoid_rampup(self.iter_num, self.max_iterations)) * math.log(2)
-        self.ramp_dev.copy_(torch.tensor([thr, cw], dtype=torch.float32))
-        return thr, cw
+    def consistency(self, out, teacher, thr, w, mask, d):
+        """the consistency of `out` against `teacher` = (ema_out, mc), uncertainty-masked by the threshold at `thr` into `mask` when
+        given -> its value (0-dim device tensor); the weight at `w` times its gradient goes to d"""
+        ema_out, mc = teacher
+        B, C, H, W = out.shape
+        cst = self.ex.buf("teacher", "cons", (3,), torch.float32)
+        call("wsl_uamt_consistency_fwd", out, ema_out, mc, self.T, B, C, H, W, thr, 0.0, mask, cst, workspace("uamt", self.dev))
+        call("wsl_uamt_consistency_bwd", out, ema_out, mask, cst, w, 0.0, B, C, H, W, d)
+        return cst[2]
+
+
+class _TwoBatchStep(_FlatSGDStep):
+    """The body the semi-supervised scripts share, on a labelled and an unlabelled batch: training forwards of the student on the
+    labelled then the unlabelled batch (BatchNorm running statistics updated in that order), the `_teacher` passes, 0.5 * (Dice + CE)
+    on the labelled batch (dense labels, CE without ignore_index), the unlabelled term of `_unsupervised` weighted by ramp_dev[0],
+    and the backward passes of the unlabelled then the labelled batch into one bucket; then SGD at the poly learning rate.
+    Two-head models use main_seg on both sides and leave the aux decoder untrained (SURVEY F7).
+
+    graph=True: one CUDA graph per batch shape after two eager warm-up steps at that shape (see `_FlatSGDStep`); the eager step
+    issues hundreds of launches from Python and is host-bound.  The script's ramps stay host arithmetic, written to ramp_dev before
+    every step.  world_size > 1: batch-sharded data parallel as `TrainStep` -- every rank runs the step on its shard, the bucket is
+    all-reduced (sum) over NCCL and the fused SGD applies the 1/world mean (world_size > 1 with graph=True: forward+backward |
+    host-issued all-reduce | SGD).  The replicas are broadcast from rank 0 at construction, a teacher once."""
+    aliases = ("parts",)
+    input_sets = 1
+    teacher = None          # a _NoisyTeacher: its passes on the unlabelled batch run before the losses
+
+    def __init__(self, model, base_lr, max_iterations, consistency, consistency_rampup, momentum, weight_decay, graph, world_size,
+                 process_group):
+        super().__init__(model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group, _aux_ids(model))
+        self.consistency, self.consistency_rampup = float(consistency), float(consistency_rampup)
+        self.ramp_dev = torch.zeros(3, dtype=torch.float32, device=self.dev)    # {consistency weight, the step's own host scalars}
+        self.parts = {}
+
+    def _ramps(self, thr=None):
+        """the consistency weight consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) of the current iteration
+        (UAMT :183, MT :164-165, EM :139) and the uncertainty threshold `thr`, written to ramp_dev -> their `parts` entries"""
+        cw = _ramp(self.consistency, self.iter_num, 300, self.consistency_rampup)
+        self.ramp_dev[:2].copy_(torch.tensor([cw, 0.0 if thr is None else thr], dtype=torch.float32))
+        return {"weight": cw, "threshold": thr}
 
     def __call__(self, image_l, label_l, image_u, noises=None):
-        """image_l/image_u: fp32 [B,1,H,W]; label_l: uint8 [B,H,W] dense.  noises (tests): list of 1 + T/2 tensors holding
-        the already-clamped noise of :147-149 and :167-169.  Returns the loss (0-dim device tensor)."""
+        """image_l/image_u: fp32 [B,1,H,W]; label_l: uint8 [B,H,W] dense.  noises (tests): list of 1 + T/2 tensors holding the
+        already-clamped noise of the teacher's inputs.  Returns the loss (0-dim device tensor)."""
         self.model.train()
-        if self.ema_model is not None:
-            self.ema_model.train()
-        thr, cw = self._ramps()
+        if self.teacher is not None:
+            self.teacher.model.train()
+        ramp_parts = self._ramps()
         assert noises is None or not self.graph_enabled, "graph mode draws the teacher noise on the device"
         loss = self._run((image_l, label_l, image_u), noises=noises)
-        self.parts = dict(self.parts, weight=cw, threshold=thr)
+        self.parts = dict(self.parts, **ramp_parts)
         return loss
+
+    def _softmax(self, logits, out):
+        """softmax over the class axis into `out` (the pCE kernel without labels)"""
+        N, C, H, W = logits.shape
+        call("wsl_softmax_pce_fwd", logits, None, out, N, C, H, W, 255, self._buf("softmax.stats", (2,)), workspace("pce", self.dev))
+
+    def _parts(self, ce, dice, supervised, term, extra):
+        return {"supervised": supervised, "consistency": term, **extra}
 
     def _fwd_bwd(self, image_l, label_l, image_u, noises=None):
         """forward passes, losses and both backward passes; returns (loss, flat gradient bucket)"""
-        ex, dev = self.ex, self.dev
-        Bl, _, H, W = image_l.shape
-        C = 4
-        self.seed_dev.add_(1)
-        masks, ck = getattr(self.model, "dropout_masks", None), getattr(self.model, "channel_keep", None)
-        outs_l, slot_l = ex.forward(image_l.contiguous(), True, True, masks, ck)
-        outs_u, slot_u = ex.forward(image_u.contiguous(), True, True, masks, ck)
-        out_l, out_u = outs_l[0], outs_u[0]
-        teacher = self._teacher(image_u, noises)
-        Bf = lambda name, shape, dt=torch.float32: ex.buf("uamt", name, shape, dt)
-        # ---- supervised half: 0.5 * (Dice + CE), CE without ignore_index (:127,:178-180) ----
-        probs, st = Bf("probs_l", (Bl, C, H, W)), Bf("stats_l", (2,))
-        call("wsl_softmax_pce_fwd", out_l, label_l, probs, Bl, C, H, W, 255, st, workspace("pce", dev))
-        sums = Bf("dice", (13,))
-        call("wsl_pdice_fwd", probs, label_l, None, 1.0, Bl, C, H, W, sums, workspace("pdice", dev))
-        gp = Bf("gprobs_l", (Bl, C, H, W))
-        call("wsl_pdice_bwd", probs, label_l, None, 1.0, sums, Bl, C, H, W, 0.5, 0, gp)
-        dl_l = Bf("dl_l", (Bl, C, H, W))
-        call("wsl_head_bwd", probs, label_l, st, None, 0.5, gp, 1.0, Bl, C, H, W, 255, dl_l, None, self.ex.dt)
-        # ---- unsupervised half (:181-189), weighted by ramp_dev[1] ----
-        cons, dl_u, mask = self._unsupervised(out_u, teacher, Bf)
-        loss = 0.5 * (sums[0] + st[0]) + self.ramp_dev[1] * cons
-        self.parts = {"supervised": 0.5 * (sums[0] + st[0]), "consistency": cons, "mask": mask}
-        # ---- two backward passes through the shared student weights, gradients accumulated in the flat bucket ----
-        nd = len(ex.dec)
-        ex.backward(slot_u, [dl_u] + [None] * (nd - 1), zero_grads=True)
-        g = ex.backward(slot_l, [dl_l] + [None] * (nd - 1), zero_grads=False)
-        return loss, g
+        ex = self.ex
+        masks = _masks(self.model)
+        outs_l, slot_l = ex.forward(image_l.contiguous(), True, True, *masks)
+        outs_u, slot_u = ex.forward(image_u.contiguous(), True, True, *masks)
+        teacher = None if self.teacher is None else self.teacher(image_u, noises)
+        dl_l = self._buf("dl_l", tuple(outs_l[0].shape))
+        ce, dice, supervised = self._ce_dice(outs_l[0], label_l, 255, self.scratch, d=dl_l)
+        term, dl_u, extra = self._unsupervised(outs_u[0], teacher)
+        loss = supervised + self.ramp_dev[0] * term
+        self.parts = self._parts(ce, dice, supervised, term, extra)
+        rest = [None] * (len(ex.dec) - 1)
+        ex.backward(slot_u, [dl_u] + rest, zero_grads=True)
+        return loss, ex.backward(slot_l, [dl_l] + rest, zero_grads=False)
 
-    def _unsupervised(self, out_u, teacher, Bf):
-        """the consistency term -> (its value, a 0-dim device tensor; w * its logit gradient; the uncertainty mask or None).
-        Threshold (:186) and weight (:183) come from ramp_dev (written by _ramps() before the body / the graph replay)."""
-        ema_out, mc = teacher
+
+class UAMTStep(_TwoBatchStep):
+    """Per-step body of train_uncertainty_aware_mean_teacher_2D.py:138-197 (BASELINE config 5) on the fused kernels.
+
+    Teacher (`ema_model`, never updated by the reference): one no-grad forward on the noisy unlabelled inputs and T/2 = 4 no-grad
+    forwards on the twice-repeated noisy batch (T = 8 stochastic passes).  The unlabelled term is the uncertainty-masked
+    softmax-MSE consistency (:181-189), weighted by w(t) = consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) (:183),
+    with the threshold of :186.  graph=True needs noises=None."""
+
+    def __init__(self, model, ema_model, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0,
+                 momentum=0.9, weight_decay=1e-4, T=8, process_group=None, world_size=1, graph=False):
+        super().__init__(model, base_lr, max_iterations, consistency, consistency_rampup, momentum, weight_decay, graph, world_size,
+                         process_group)
+        self.ema_model = ema_model
+        self.teacher = _NoisyTeacher(ema_model, T, self.dev, self.world_size, self.pg)
+
+    def _ramps(self):
+        thr = (0.75 + 0.25 * ramps.sigmoid_rampup(self.iter_num, self.max_iterations)) * math.log(2)       # :186
+        return super()._ramps(thr if self.teacher.T else None)
+
+    def _unsupervised(self, out_u, teacher):
+        """the consistency term -> (its value, w * its logit gradient, {"mask": the uncertainty mask or None})"""
         B, C, H, W = out_u.shape
-        mask, cst = (Bf("mask", (B, H, W), torch.uint8) if self.T else None), Bf("cons", (3,))
-        call("wsl_uamt_consistency_fwd", out_u, ema_out, mc, self.T, B, C, H, W, self.ramp_dev[0:1], 0.0, mask, cst,
-             workspace("uamt", self.dev))
-        dl_u = Bf("dl_u", (B, C, H, W))
-        call("wsl_uamt_consistency_bwd", out_u, ema_out, mask, cst, self.ramp_dev[1:2], 0.0, B, C, H, W, dl_u)
-        return cst[2], dl_u, mask
+        mask = self._buf("mask", (B, H, W), torch.uint8) if self.teacher.T else None
+        dl_u = self._buf("dl_u", (B, C, H, W))
+        cons = self.teacher.consistency(out_u, teacher, self.ramp_dev[1:2], self.ramp_dev[0:1], mask, dl_u)
+        return cons, dl_u, {"mask": mask}
 
 
 class MeanTeacherStep(UAMTStep):
-    """Per-step body of train_mean_teacher_2D.py:138-180 on the fused kernels: `UAMTStep` without the uncertainty estimate.
+    """Per-step body of train_mean_teacher_2D.py:138-180 on the fused kernels: `UAMTStep` with T = 0, no uncertainty estimate.
 
-    Student: training forwards with gradient on the labelled then the unlabelled batch (two BatchNorm batches, running statistics
-    updated in that order).  Teacher (`ema_model`): one training-mode no-grad forward on unlabelled + clamp(0.1 * randn, +-0.2)
-    (:147-149, :157-159).  Loss = 0.5 * (Dice + CE) on the labelled batch (dense labels, CE without ignore_index, :127) +
-    w(t) * torch.mean((softmax(student_u) - softmax(teacher))^2) (:169-170, the consistency kernels' T = 0 mode) with
-    w(t) = consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) (:73-75, :164-165); two backward passes into one
-    bucket, then SGD at the poly learning rate.  As written in the script, the teacher is never updated and never put in eval
-    mode (update_ema_variables is defined but not called, SURVEY F8).
-
-    graph=True: one CUDA graph per batch shape after two eager warm-up steps at that shape (see `_FlatSGDStep`); the ramp weight
-    is read from device memory.  world_size > 1: batch-sharded data parallel as `UAMTStep` (teacher broadcast once).  Two-head
-    models use main_seg on both sides (SURVEY F7)."""
+    Teacher (`ema_model`): one training-mode no-grad forward on unlabelled + clamp(0.1 * randn, +-0.2) (:147-149, :157-159).  The
+    unlabelled term is torch.mean((softmax(student_u) - softmax(teacher))^2) (:169-170, the consistency kernels' T = 0 mode),
+    weighted by w(t) = consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) (:73-75, :164-165).  As written in the
+    script, the teacher is never updated and never put in eval mode (update_ema_variables is defined but not called, SURVEY F8)."""
 
     def __init__(self, model, ema_model, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0,
                  momentum=0.9, weight_decay=1e-4, world_size=1, process_group=None, graph=False, global_batch=False):
@@ -587,65 +624,59 @@ class MeanTeacherStep(UAMTStep):
                          consistency_rampup=consistency_rampup, momentum=momentum, weight_decay=weight_decay, T=0,
                          process_group=process_group, world_size=world_size, graph=graph)
 
-    def _ramps(self):
-        """the consistency weight of :164-165 -> (None: no threshold, weight), also written to ramp_dev[1]"""
-        cw = self.consistency * self.ramps.sigmoid_rampup(self.iter_num // 300, self.consistency_rampup)
-        self.ramp_dev.copy_(torch.tensor([0.0, cw], dtype=torch.float32))
-        return None, cw
 
+class EntropyMinStep(_TwoBatchStep):
+    """Per-step body of train_entropy_minimization_2D.py:121-150 on the fused kernels, with no teacher.
 
-class EntropyMinStep(UAMTStep):
-    """Per-step body of train_entropy_minimization_2D.py:121-150 on the fused kernels.
-
-    The student forwards and the supervised half of `MeanTeacherStep` (no teacher); the unsupervised term is
-    w(t) * losses.entropy_loss(softmax(student_u), C=4) (:141, utils/losses.py:30-36) with the same ramp
-    w(t) = consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) (:139).  graph=True and world_size > 1 as
-    `MeanTeacherStep`."""
-    _ramps = MeanTeacherStep._ramps
+    The unlabelled term is losses.entropy_loss(softmax(student_u), C=4) (:141, utils/losses.py:30-36), weighted by
+    w(t) = consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) (:139)."""
 
     def __init__(self, model, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0, momentum=0.9,
                  weight_decay=1e-4, world_size=1, process_group=None, graph=False, global_batch=False):
         if global_batch:
             raise NotImplementedError("global_batch semantics are not defined for the entropy-minimisation step (run it with per-rank normalisers)")
-        super().__init__(model, None, base_lr=base_lr, max_iterations=max_iterations, consistency=consistency,
-                         consistency_rampup=consistency_rampup, momentum=momentum, weight_decay=weight_decay, T=0,
-                         process_group=process_group, world_size=world_size, graph=graph)
+        super().__init__(model, base_lr, max_iterations, consistency, consistency_rampup, momentum, weight_decay, graph, world_size,
+                         process_group)
 
-    def _teacher(self, img, noises):
-        return None
-
-    def _unsupervised(self, out_u, teacher, Bf):
+    def _unsupervised(self, out_u, teacher):
         B, C, H, W = out_u.shape
-        probs, ent = Bf("probs_u", (B, C, H, W)), Bf("ent", (1,))
-        call("wsl_softmax_pce_fwd", out_u, None, probs, B, C, H, W, 255, Bf("stats_u", (2,)), workspace("pce", self.dev))
+        probs, ent = self._buf("probs_u", (B, C, H, W)), self._buf("ent", (1,))
+        self._softmax(out_u, probs)
         call("wsl_entropy_fwd", probs, B, C, H, W, ent, workspace("ent", self.dev))
-        gp, dl_u = Bf("gprobs_u", (B, C, H, W)), Bf("dl_u", (B, C, H, W))
+        gp, dl_u = self._buf("gprobs_u", (B, C, H, W)), self._buf("dl_u", (B, C, H, W))
         call("wsl_entropy_bwd", probs, B, C, H, W, 1.0, 0, gp)
         # the ramp weight scales the probability gradient from device memory, so one captured graph serves every iteration
         # (wsl_entropy_bwd takes its scale as a launch argument, and wsl_head_bwd's grad_out scales the CE term only)
-        gp.mul_(self.ramp_dev[1])
+        gp.mul_(self.ramp_dev[0])
         call("wsl_head_bwd", probs, None, None, None, 0.0, gp, 1.0, B, C, H, W, 255, dl_u, None, self.ex.dt)
-        return ent[0], dl_u, None
+        return ent[0], dl_u, {"mask": None}
 
 
-class USTMStep(UAMTStep):
+class USTMStep(_FlatSGDStep):
     """Per-step body of train_weakly_supervised_ustm_2D.py:113-170: pCE on scribbles + uncertainty-aware self-ensembling with a
-    random rot90 transform (Python host RNG, :123) and the EMA teacher update the script really performs (:163).
+    random rot90 transform (Python host RNG, :123) and the EMA teacher update the script really performs (:163).  The teacher's
+    passes and the consistency are `UAMTStep`'s, on the rotated batch.
 
     graph=True: the rot90 count is a kernel ARGUMENT, so one CUDA graph is captured per count (at most four, each on the first
     step that draws it after two eager warm-up steps); threshold, consistency weight and the EMA factor reach the captured
     kernels through `ramp_dev`."""
+    aliases = ("parts",)
+    input_sets = 1          # graphs are keyed by the rot90 count alone
 
-    def __init__(self, model, ema_model, base_lr=0.01, max_iterations=60000, ema_decay=0.99, **kw):
-        super().__init__(model, ema_model, base_lr=base_lr, max_iterations=max_iterations, **kw)
+    def __init__(self, model, ema_model, base_lr=0.01, max_iterations=60000, ema_decay=0.99, *, consistency=0.1,
+                 consistency_rampup=200.0, momentum=0.9, weight_decay=1e-4, T=8, process_group=None, world_size=1, graph=False):
+        """The keywords after ema_decay are `UAMTStep`'s; consistency and consistency_rampup are accepted and unused (the script's
+        weight ramp is fixed, :145)."""
+        super().__init__(model, base_lr, max_iterations, momentum, weight_decay, graph, world_size, process_group, _aux_ids(model))
+        self.ema_model = ema_model
+        self.teacher = _NoisyTeacher(ema_model, T, self.dev, self.world_size, self.pg)
         self.ema_decay = float(ema_decay)
-        self.tflat, _ = _flatten(self.ex_t.params, self.dev)
+        self.tflat, _ = _flatten(self.teacher.ex.params, self.dev)
         self.ramp_dev = torch.zeros(3, dtype=torch.float32, device=self.dev)     # {threshold, weight, 1 - EMA alpha}
 
     def _ramps(self):
-        import math
-        cw = 1.0 * self.ramps.sigmoid_rampup(self.iter_num // 1000, 60)                                      # :145
-        thr = (0.75 + 0.25 * self.ramps.sigmoid_rampup(self.iter_num, self.max_iterations)) * math.log(2)     # :148
+        cw = _ramp(1.0, self.iter_num, 1000, 60)                                 # :145
+        thr = (0.75 + 0.25 * ramps.sigmoid_rampup(self.iter_num, self.max_iterations)) * math.log(2)     # :148
         alpha = min(1 - 1 / (self.iter_num + 1), self.ema_decay)         # :63, global_step = iter_num before the increment
         self.ramp_dev.copy_(torch.tensor([thr, cw, 1.0 - alpha], dtype=torch.float32))
         return thr, cw, alpha
@@ -671,32 +702,25 @@ class USTMStep(UAMTStep):
         return loss
 
     def _fwd_bwd(self, image, label, noises=None):
-        ex, dev = self.ex, self.dev
-        B, _, H, W = image.shape
-        C, T, k = 4, self.T, self.rot_times
-        self.seed_dev.add_(1)
-        masks, ck = getattr(self.model, "dropout_masks", None), getattr(self.model, "channel_keep", None)
-        outs, slot = ex.forward(image.contiguous(), True, True, masks, ck)
+        ex, dev, k = self.ex, self.dev, self.rot_times
+        outs, slot = ex.forward(image.contiguous(), True, True, *_masks(self.model))
         out = outs[0]
-        Bf = lambda name, shape, dt=torch.float32: ex.buf("ustm", name, shape, dt)
-        rimg = Bf("rimg", (B, 1, H, W))
+        B, C, H, W = out.shape
+        rimg = self._buf("rimg", (B, 1, H, W))
         call("wsl_rot90", image.contiguous(), B, H, k, 0, rimg)
-        ema_out, mc = self._teacher(rimg, noises)
+        teacher = self.teacher(rimg, noises)
         # pCE (ignore_index 4)
-        probs, st = Bf("probs", (B, C, H, W)), Bf("stats", (2,))
+        probs, st = self._buf("probs", (B, C, H, W)), self._buf("stats", (2,))
         call("wsl_softmax_pce_fwd", out, label, probs, B, C, H, W, 4, st, workspace("pce", dev))
-        d = Bf("dl", (B, C, H, W))
+        d = self._buf("dl", (B, C, H, W))
         call("wsl_head_bwd", probs, label, st, None, 1.0, None, 0.0, B, C, H, W, 4, d, None, self.ex.dt)
         # consistency on the rotated student logits; threshold (:148) / weight (:145) from ramp_dev
-        rout = Bf("rout", (B, C, H, W))
+        rout, dr, mask = self._buf("rout", (B, C, H, W)), self._buf("dr", (B, C, H, W)), self._buf("mask", (B, H, W), torch.uint8)
         call("wsl_rot90", out, B * C, H, k, 0, rout)
-        mask, cst = Bf("mask", (B, H, W), torch.uint8), Bf("cons", (3,))
-        call("wsl_uamt_consistency_fwd", rout, ema_out, mc, T, B, C, H, W, self.ramp_dev[0:1], 0.0, mask, cst, workspace("uamt", dev))
-        dr = Bf("dr", (B, C, H, W))
-        call("wsl_uamt_consistency_bwd", rout, ema_out, mask, cst, self.ramp_dev[1:2], 0.0, B, C, H, W, dr)
+        cons = self.teacher.consistency(rout, teacher, self.ramp_dev[0:1], self.ramp_dev[1:2], mask, dr)
         call("wsl_rot90", dr, B * C, H, (4 - k) % 4, 1, d)              # rotate the gradient back and add it to the pCE part
-        loss = st[0] + self.ramp_dev[1] * cst[2]
-        self.parts = {"ce": st[0], "consistency": cst[2], "mask": mask}
+        loss = st[0] + self.ramp_dev[1] * cons
+        self.parts = {"ce": st[0], "consistency": cons, "mask": mask}
         g = ex.backward(slot, [d] + [None] * (len(ex.dec) - 1))
         return loss, g
 
@@ -781,14 +805,13 @@ class S2LStep(TrainStep):
             call("wsl_s2l_refresh", outs[0], tab, B, size, max_hw, a, b, store.weight_live)
 
 
-class DANStep(_FlatSGDStep):
+class DANStep(_TwoBatchStep):
     """Per-step body of train_deep_adversarial_network_2D.py:126-184 (adversarial semi-supervised training with FCDiscriminator).
 
-    Phase 1 (`_fwd_bwd`, :138-160; student in training mode, D in eval mode): training forwards of the labelled then the unlabelled
-    half (BatchNorm running statistics updated in that order), 0.5 * (Dice + CE) on the labelled half (CE without ignore_index), and
-    w(t) * CE(D(softmax(out_u), image_u), DAN_target[:B_u]) with w(t) = consistency * sigmoid_rampup(iter_num // 150, rampup).  That
-    term reaches the student through D's map gradient and the softmax Jacobian; D's own parameter gradients, which the script
-    discards (:176), are not computed.  Then SGD (momentum 0.9, weight decay 1e-4) at the poly learning rate.
+    Phase 1 (`_fwd_bwd`, :138-160; student in training mode, D in eval mode): the two-batch body of `_TwoBatchStep` with the
+    unlabelled term w(t) * CE(D(softmax(out_u), image_u), DAN_target[:B_u]), w(t) = consistency * sigmoid_rampup(iter_num // 150,
+    rampup).  That term reaches the student through D's map gradient and the softmax Jacobian; D's own parameter gradients, which
+    the script discards (:176), are not computed.  Then SGD (momentum 0.9, weight decay 1e-4) at the poly learning rate.
     Phase 2 (`_finish`, :162-178; student in eval mode, D in training mode with fresh Dropout2d masks): no-grad eval forwards of both
     halves on the updated weights, D on cat(softmax_l, softmax_u) against [1]*B_l + [0]*B_u, and one Adam step of D
     (`wsl_adam_step`, torch's multi-tensor arithmetic) over D's parameters, which live in one flat buffer (`dflat`).
@@ -798,8 +821,7 @@ class DANStep(_FlatSGDStep):
     the whole iteration as one CUDA graph per batch shape after two eager warm-up steps at that shape: the first batch, a full one
     with B_u == B_l, and after it an epoch's shorter last batches; the ramp weight and Adam's t-dependent scalars are written to `ramp_dev` before every step.  The modules' train() / eval() flags are not touched: each pass runs in the script's mode.
     Test hooks: `model.dropout_masks` (phase 1) and `disc.channel_keep` (phase 2, [B_l + B_u, C] masks) as for the modules."""
-    aliases = ("parts",)
-    input_sets = 1
+    scratch = "dan"
 
     def __init__(self, model, disc, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0, disc_lr=1e-4,
                  betas=(0.9, 0.99), graph=True, world_size=1):
@@ -809,12 +831,7 @@ class DANStep(_FlatSGDStep):
         if len(getattr(ex, "dec", ())) != 1 or any(getattr(ex, "ds_heads", ())):
             raise ValueError("DANStep needs a single-output segmentation network: the script takes torch.softmax(model(x), dim=1) "
                              "(train_deep_adversarial_network_2D.py:143-144), which fails on a tuple of outputs")
-        from .utils import ramps
-        super().__init__(model, base_lr, max_iterations, 0.9, 1e-4, graph, 1, None)
-        self.ramps = ramps
-        self.segments = [[0, self.flat.numel()]]
-        self.n_trained = self.flat.numel()
-        self.consistency, self.consistency_rampup = float(consistency), float(consistency_rampup)
+        super().__init__(model, base_lr, max_iterations, consistency, consistency_rampup, 0.9, 1e-4, graph, 1, None)
         self.disc, self.dex = disc, disc.executor
         if next(disc.parameters()).device != self.dev:
             raise ValueError(f"DANStep: the discriminator is on {next(disc.parameters()).device}, the model on {self.dev}")
@@ -823,8 +840,6 @@ class DANStep(_FlatSGDStep):
         self.exp_avg, self.exp_avg_sq = torch.zeros_like(self.dflat), torch.zeros_like(self.dflat)
         self.adam_t = 0
         self.disc_lr, self.betas, self.eps = float(disc_lr), (float(betas[0]), float(betas[1])), 1e-8
-        self.ramp_dev = torch.zeros(3, dtype=torch.float32, device=self.dev)   # {ramp weight, lr / (1 - b1^t), sqrt(1 - b2^t)}
-        self.parts = {}
 
     def __call__(self, image_l, label_l, image_u):
         """image_l / image_u: fp32 [B_l,1,256,256] / [B_u,1,256,256]; label_l: uint8 [B_l,256,256] dense.  Returns the phase-1 loss
@@ -840,7 +855,7 @@ class DANStep(_FlatSGDStep):
             raise ValueError(f"DANStep(graph=True) takes its first batch as the full batch and needs B_u == B_l there (got "
                              f"{image_u.shape[0]} and {image_l.shape[0]}); an epoch's shorter last batches may follow, each captured "
                              f"in its own graph")
-        cw = self.consistency * self.ramps.sigmoid_rampup(self.iter_num // 150, self.consistency_rampup)     # :151-152
+        cw = _ramp(self.consistency, self.iter_num, 150, self.consistency_rampup)     # :151-152
         t = self.adam_t + 1
         b1, b2 = self.betas
         step_size, bc2_sqrt = self.disc_lr / (1 - b1 ** t), (1 - b2 ** t) ** 0.5          # as torch's Adam computes them (doubles)
@@ -850,63 +865,43 @@ class DANStep(_FlatSGDStep):
         self.parts = dict(self.parts, weight=cw)
         return loss
 
-    def _softmax(self, logits, out, name):
-        N, C, H, W = logits.shape
-        call("wsl_softmax_pce_fwd", logits, None, out, N, C, H, W, 255, self.ex.buf("dan", name, (2,), torch.float32),
-             workspace("pce", self.dev))
-
     def _fwd_bwd(self, image_l, label_l, image_u):
         """phase 1 -> (loss, student gradient bucket)"""
-        ex, dex, dev = self.ex, self.dex, self.dev
-        B, _, H, W = image_l.shape
-        Bu, C = image_u.shape[0], 4
         self._inputs = (image_l, image_u)
-        self._dpacks = dex.pack_resident(dev)
-        masks, ck = getattr(self.model, "dropout_masks", None), getattr(self.model, "channel_keep", None)
-        outs_l, slot_l = ex.forward(image_l.contiguous(), True, True, masks, ck)
-        outs_u, slot_u = ex.forward(image_u.contiguous(), True, True, masks, ck)
-        Bf = lambda name, shape, dt=torch.float32: ex.buf("dan", name, shape, dt)
-        # ---- supervised half: 0.5 * (Dice + CE) (:146-149), CE without ignore_index ----
-        probs, st = Bf("probs_l", (B, C, H, W)), Bf("stats_l", (2,))
-        call("wsl_softmax_pce_fwd", outs_l[0], label_l, probs, B, C, H, W, 255, st, workspace("pce", dev))
-        sums = Bf("dice", (13,))
-        call("wsl_pdice_fwd", probs, label_l, None, 1.0, B, C, H, W, sums, workspace("pdice", dev))
-        gp = Bf("gprobs_l", (B, C, H, W))
-        call("wsl_pdice_bwd", probs, label_l, None, 1.0, sums, B, C, H, W, 0.5, 0, gp)
-        dl_l = Bf("dl_l", (B, C, H, W))
-        call("wsl_head_bwd", probs, label_l, st, None, 0.5, gp, 1.0, B, C, H, W, 255, dl_l, None, ex.dt)
-        # ---- adversarial term (:151-157): D in eval mode on softmax(out_u); its gradient w.r.t. the map only ----
-        pu = Bf("probs_u", (Bu, C, H, W))
-        self._softmax(outs_u[0], pu, "stats_u")
-        logits, rec = dex.forward(pu, image_u.contiguous(), False, True, True, None, packs=self._dpacks)
-        adv, dlg = Bf("adv", (1,)), Bf("dlogits_u", (Bu, 2))
+        self._dpacks = self.dex.pack_resident(self.dev)
+        return super()._fwd_bwd(image_l, label_l, image_u)
+
+    def _unsupervised(self, out_u, teacher):
+        """the adversarial term (:151-157): D in eval mode on softmax(out_u); its gradient w.r.t. the map only"""
+        B, Bu = self._inputs[0].shape[0], out_u.shape[0]
+        _, C, H, W = out_u.shape
+        pu = self._buf("probs_u", (Bu, C, H, W))
+        self._softmax(out_u, pu)
+        logits, rec = self.dex.forward(pu, self._inputs[1].contiguous(), False, True, True, None, packs=self._dpacks)
+        adv, dlg = self._buf("adv", (1,)), self._buf("dlogits_u", (Bu, 2))
         call("wsl_disc_ce", logits, Bu, min(B, Bu), self.ramp_dev[0:1], 0.0, adv, dlg)
-        dmap, _, _ = dex.backward(rec, dlg, True, False, param_grads=False)
-        dl_u = Bf("dl_u", (Bu, C, H, W))
-        call("wsl_head_bwd", pu, None, None, None, 0.0, dmap, 1.0, Bu, C, H, W, 255, dl_u, None, ex.dt)
-        loss = 0.5 * (sums[0] + st[0]) + self.ramp_dev[0] * adv[0]
-        self.parts = {"loss_ce": st[0], "loss_dice": sums[0], "consistency": adv[0]}
-        # ---- both backward passes through the shared student weights, accumulated in the flat bucket ----
-        ex.backward(slot_u, [dl_u], zero_grads=True)
-        g = ex.backward(slot_l, [dl_l], zero_grads=False)
-        return loss, g
+        dmap, _, _ = self.dex.backward(rec, dlg, True, False, param_grads=False)
+        dl_u = self._buf("dl_u", (Bu, C, H, W))
+        call("wsl_head_bwd", pu, None, None, None, 0.0, dmap, 1.0, Bu, C, H, W, 255, dl_u, None, self.ex.dt)
+        return adv[0], dl_u, {}
+
+    def _parts(self, ce, dice, supervised, term, extra):
+        return {"loss_ce": ce, "loss_dice": dice, "consistency": term}
 
     def _finish(self, g, captured):
         """student SGD (:158-160), then phase 2 (:162-178) and D's Adam step; host scalars come from ramp_dev in both modes"""
         self._opt(g)
-        ex, dex, dev = self.ex, self.dex, self.dev
+        ex, dex = self.ex, self.dex
         image_l, image_u = self._inputs
         B, _, H, W = image_l.shape
-        Bu, C = image_u.shape[0], 4
-        N = B + Bu
-        Bf = lambda name, shape, dt=torch.float32: ex.buf("dan", name, shape, dt)
-        maps, imgs = Bf("maps", (N, C, H, W)), Bf("imgs", (N, 1, H, W))
-        self._softmax(ex.forward(image_l.contiguous(), False, False)[0][0], maps[:B], "stats_e")
-        self._softmax(ex.forward(image_u.contiguous(), False, False)[0][0], maps[B:], "stats_e")
+        N = B + image_u.shape[0]
+        maps, imgs = self._buf("maps", (N, ex.n_class, H, W)), self._buf("imgs", (N, 1, H, W))
+        self._softmax(ex.forward(image_l.contiguous(), False, False)[0][0], maps[:B])
+        self._softmax(ex.forward(image_u.contiguous(), False, False)[0][0], maps[B:])
         imgs[:B].copy_(image_l)
         imgs[B:].copy_(image_u)
         logits, rec = dex.forward(maps, imgs, True, True, False, getattr(self.disc, "channel_keep", None), packs=self._dpacks)
-        dloss, dlg = Bf("disc_loss", (1,)), Bf("dlogits_d", (N, 2))
+        dloss, dlg = self._buf("disc_loss", (1,)), self._buf("dlogits_d", (N, 2))
         call("wsl_disc_ce", logits, N, B, None, 1.0, dloss, dlg)
         dex.backward(rec, dlg, False, False, bucket=(self.dgrad, self.doffsets))
         b1, b2 = self.betas
