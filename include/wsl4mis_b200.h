@@ -130,6 +130,11 @@ int wsl_add_clamped_noise(const float* x, long long n, int reps, float sigma, fl
 int wsl_zoom_nearest(const void* src, int is_u8, int S, int h, int w, int H, int W, void* dst, cudaStream_t stream);
 int wsl_overlap_counts(const uint8_t* pred, const uint8_t* gt, long long n, int classes, unsigned long long* counts_zeroed,
                        cudaStream_t stream);
+/* The same resize for N slices of their own sizes (the resident validation set): table = device int64 [N][3] rows {element
+ * offset of the slice in the ragged store, h, w}.  dir 0: ragged src (slice s at table[s], h x w) -> dense dst [N,H,W];
+ * dir 1: dense src [N,H,W] -> ragged dst (slice s back to its h x w at table[s]).  max_hw >= every h*w; N <= 65535. */
+int wsl_zoom_nearest_ragged(const void* src, int is_u8, const long long* table, int N, int max_hw, int dir, int H, int W,
+                            void* dst, cudaStream_t stream);
 
 /* torch.rot90(x, k, [2,3]) of square fp32 maps ([planes,S,S]; dst (+)= rot(src)) and the mean-teacher EMA update
  * ema = alpha*ema + (1-alpha)*param (train_weakly_supervised_ustm_2D.py:61-65,124-125,150,163). */
@@ -190,6 +195,18 @@ int wsl_random_walker(const float* images, const uint8_t* scribbles, const long 
 int wsl_surface_metrics_workspace(int ndim, int S, int H, int W, int classes, long long* out_bytes);
 int wsl_surface_metrics(const uint8_t* pred, const uint8_t* gt, int ndim, int S, int H, int W, int classes, double sz, double sy,
                         double sx, void* ws, double* out, cudaStream_t stream);
+/* The same metrics for V volumes of different shapes in one launch sequence, bit-identical to V wsl_surface_metrics calls:
+ * pred / gt hold the volumes back to back; vols is a device table of V rows of wsl_surface_metrics_volume_bytes() bytes,
+ *   {int64 voff, roff, coff; int32 S, H, W, rank3; double sz, sy, sx},
+ * the volume's first voxel, first x-row (prefix of S*H) and first (y, x) column (prefix of H*W) in the set, its shape (rank3 0:
+ * an [H,W] volume with S = 1) and spacing.  Totals: n_total voxels, rows_total x-rows, cols_total columns; max_n / max_w the
+ * largest volume's voxels / W (each volume within wsl_surface_metrics' limits; V <= 65535).  out: [V, classes-1, 12] doubles,
+ * the single-volume rows per volume.  ws: wsl_surface_metrics_batched_workspace() bytes, 256-byte aligned, no zeroing needed. */
+int wsl_surface_metrics_volume_bytes(void);
+int wsl_surface_metrics_batched_workspace(int V, long long n_total, long long rows_total, int classes, long long* out_bytes);
+int wsl_surface_metrics_batched(const uint8_t* pred, const uint8_t* gt, const void* vols, int V, long long n_total, long long rows_total,
+                                long long cols_total, long long max_n, int max_w, int classes, void* ws, double* out,
+                                cudaStream_t stream);
 
 /* ---- network operators (networks/unet.py) ---------------------------------------------------------------- */
 

@@ -2,6 +2,8 @@
 // Each kernel cites the reference lines (relative to /root/reference/code) whose result it reproduces.
 #include "common.cuh"
 
+#include <algorithm>
+
 namespace {
 
 constexpr int C4 = 4;
@@ -669,6 +671,27 @@ __global__ void __launch_bounds__(TPB) zoom_nearest_kernel(const T* __restrict__
   }
 }
 
+// The same resize for slices of different sizes, listed in a table of {element offset in the ragged store, h, w} rows (int64).
+// dir 0: every slice s, read at table[s] from the ragged `src`, -> dense dst[s] of H x W; dir 1: dense src[s] of H x W -> the
+// slice's own h x w at table[s] in the ragged `dst`.  blockIdx.y = slice.
+template <typename T>
+__global__ void __launch_bounds__(TPB) zoom_nearest_ragged_kernel(const T* __restrict__ src, const long long* __restrict__ table, int dir,
+                                                                  int H, int W, T* __restrict__ dst) {
+  const long long* row = table + 3 * (long long)blockIdx.y;
+  const long long off = row[0];
+  const int h = (int)row[1], w = (int)row[2];
+  const int ih = dir ? H : h, iw = dir ? W : w, oh = dir ? h : H, ow = dir ? w : W;
+  const T* in = src + (dir ? (long long)blockIdx.y * H * W : off);
+  T* out = dst + (dir ? off : (long long)blockIdx.y * H * W);
+  const long long total = (long long)oh * ow;
+  for (long long i = blockIdx.x * (long long)TPB + threadIdx.x; i < total; i += (long long)gridDim.x * TPB) {
+    const int x = (int)(i % ow), y = (int)(i / ow);
+    bool oy, ox;
+    const int iy = zoom0_index(y, ih, oh, oy), ix = zoom0_index(x, iw, ow, ox);
+    out[i] = (oy || ox) ? (T)0 : in[(long long)iy * iw + ix];
+  }
+}
+
 // counts[c] = {|pred==c & gt==c|, |pred==c|, |gt==c|} for c = 1..classes-1 (medpy.metric.binary.dc inputs)
 __global__ void __launch_bounds__(TPB) overlap_counts_kernel(const uint8_t* __restrict__ pred, const uint8_t* __restrict__ gt,
                                                              long long n, int classes, unsigned long long* __restrict__ counts) {
@@ -1164,6 +1187,19 @@ WSL_API int wsl_zoom_nearest(const void* src, int is_u8, int S, int h, int w, in
   if (is_u8) zoom_nearest_kernel<uint8_t><<<grid_for(total, TPB), TPB, 0, stream>>>((const uint8_t*)src, S, h, w, H, W, (uint8_t*)dst);
   else zoom_nearest_kernel<float><<<grid_for(total, TPB), TPB, 0, stream>>>((const float*)src, S, h, w, H, W, (float*)dst);
   return wsl_check_launch("zoom_nearest");
+}
+
+WSL_API int wsl_zoom_nearest_ragged(const void* src, int is_u8, const long long* table, int N, int max_hw, int dir, int H, int W,
+                                    void* dst, cudaStream_t stream) {
+  WSL_REQUIRE(N >= 1 && N <= 65535 && (dir == 0 || dir == 1) && H >= 1 && W >= 1 && max_hw >= 1,
+              "wsl_zoom_nearest_ragged: N in 1..65535, dir 0 or 1, positive sizes (got N=%d, dir=%d, %dx%d, max_hw=%d)", N, dir, H, W, max_hw);
+  const long long per = dir ? (long long)max_hw : (long long)H * W;       // output elements of the largest slice
+  const dim3 grid((unsigned)std::min<long long>((per + TPB - 1) / TPB, 1024), (unsigned)N);
+  if (is_u8)
+    zoom_nearest_ragged_kernel<uint8_t><<<grid, TPB, 0, stream>>>((const uint8_t*)src, table, dir, H, W, (uint8_t*)dst);
+  else
+    zoom_nearest_ragged_kernel<float><<<grid, TPB, 0, stream>>>((const float*)src, table, dir, H, W, (float*)dst);
+  return wsl_check_launch("zoom_nearest_ragged");
 }
 
 WSL_API int wsl_overlap_counts(const uint8_t* pred, const uint8_t* gt, long long n, int classes, unsigned long long* counts_zeroed,

@@ -347,6 +347,7 @@ class TrainStep(_FlatSGDStep):
             probs.append(p)
             stats.append(st)
         ce = stats[0][0]
+        self.loss_parts = {"ce": ce}
         if v == "pce":
             loss = ce
             dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, None, 0.0 * S, slot)
@@ -365,6 +366,7 @@ class TrainStep(_FlatSGDStep):
             call("wsl_mumford_shah_bwd", image, probs[0], cent, N, C, H, W, 1e-6, 0, gp)
             loss = ce + 1e-6 * out[0]
             dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, 1.0 * S, slot)
+            self.loss_parts["ms"] = out[0]
         elif v == "pce_tv":
             # tv_loss(outputs_soft[1:]) -- batch slice, sample 0 gets no TV term (SURVEY F12)
             gp = B("gprobs0", (N, C, H, W))
@@ -373,6 +375,7 @@ class TrainStep(_FlatSGDStep):
             if N > 1:
                 call("wsl_tv_loss", probs[0][1:], (N - 1) * C, H, W, 1e-2, gp[1:], out, workspace("tv", dev))
                 loss = ce + 1e-2 * out[0]
+                self.loss_parts["tv"] = out[0]
             else:
                 loss = ce   # mean over an empty tensor is NaN in the reference; N=1 is never used with this script
             dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, 1.0 * S, slot)
@@ -383,6 +386,7 @@ class TrainStep(_FlatSGDStep):
             call("wsl_entropy_bwd", probs[0], N, C, H, W, 0.1, 0, gp)
             loss = ce + 0.1 * out[0]
             dl[0] = self._head_bwd(0, probs, stats, label, 1.0 * S, gp, 1.0 * S * G, slot)
+            self.loss_parts["entropy"] = out[0]
         elif v == "pce_variance":
             w = _ramp(self.consistency, self.iter_num, 150, self.consistency_rampup)
             gp = B("gprobs0", (N, C, H, W))
@@ -398,6 +402,7 @@ class TrainStep(_FlatSGDStep):
             pseudo = B("pseudo", (N, H, W), torch.uint8)
             call("wsl_mix_argmax", probs[0], probs[1], 0.0, 0.0, self.beta_dev, N, C, H, W, pseudo)   # beta from device memory
             loss = 0.5 * (stats[0][0] + stats[1][0])
+            self.loss_parts = {"ce": loss}
             # pDLoss weighs every pixel by the batch-summed ignore mask (F14); with pseudo labels nothing is ignored, so the weight
             # is the batch size -- the GLOBAL one when the ranks reproduce the single-process arithmetic
             nb = float(N * self.world_size) if self.global_batch else float(N)
@@ -412,6 +417,7 @@ class TrainStep(_FlatSGDStep):
                 call("wsl_pdice_bwd", probs[h], pseudo, None, nb, sums, N, C, H, W, 0.25, 0, gp)
                 loss = loss + 0.25 * sums[0]
                 dl[h] = self._head_bwd(h, probs, stats, label, 0.5 * S, gp, 1.0 * S, slot)
+            self.loss_parts["pse_sup"] = 0.5 * (B("pd0", (13,))[0] + B("pd1", (13,))[0])
         return loss, dl
 
     def _fwd_bwd(self, image, label):
@@ -457,7 +463,7 @@ class TrainStep(_FlatSGDStep):
             # beta = random.random() + 1e-10 from Python's host RNG, as the script (:117); handed to the kernels through
             # device memory so the captured graph sees a fresh value every replay
             self.beta = random.random() + 1e-10
-            self.beta_dev.copy_(torch.tensor([self.beta, 1.0 - self.beta], dtype=torch.float32), non_blocking=False)
+            self.beta_dev.copy_(torch.tensor([self.beta, 1.0 - self.beta], dtype=torch.float32), non_blocking=True)
         return self._run((image, label))
 
     @property
@@ -540,7 +546,7 @@ class _TwoBatchStep(_FlatSGDStep):
         """the consistency weight consistency * sigmoid_rampup(iter_num // 300, consistency_rampup) of the current iteration
         (UAMT :183, MT :164-165, EM :139) and the uncertainty threshold `thr`, written to ramp_dev -> their `parts` entries"""
         cw = _ramp(self.consistency, self.iter_num, 300, self.consistency_rampup)
-        self.ramp_dev[:2].copy_(torch.tensor([cw, 0.0 if thr is None else thr], dtype=torch.float32))
+        self.ramp_dev[:2].copy_(torch.tensor([cw, 0.0 if thr is None else thr], dtype=torch.float32), non_blocking=True)
         return {"weight": cw, "threshold": thr}
 
     def __call__(self, image_l, label_l, image_u, noises=None):
@@ -561,7 +567,7 @@ class _TwoBatchStep(_FlatSGDStep):
         call("wsl_softmax_pce_fwd", logits, None, out, N, C, H, W, 255, self._buf("softmax.stats", (2,)), workspace("pce", self.dev))
 
     def _parts(self, ce, dice, supervised, term, extra):
-        return {"supervised": supervised, "consistency": term, **extra}
+        return {"loss_ce": ce, "loss_dice": dice, "supervised": supervised, "consistency": term, **extra}
 
     def _fwd_bwd(self, image_l, label_l, image_u, noises=None):
         """forward passes, losses and both backward passes; returns (loss, flat gradient bucket)"""
@@ -678,7 +684,7 @@ class USTMStep(_FlatSGDStep):
         cw = _ramp(1.0, self.iter_num, 1000, 60)                                 # :145
         thr = (0.75 + 0.25 * ramps.sigmoid_rampup(self.iter_num, self.max_iterations)) * math.log(2)     # :148
         alpha = min(1 - 1 / (self.iter_num + 1), self.ema_decay)         # :63, global_step = iter_num before the increment
-        self.ramp_dev.copy_(torch.tensor([thr, cw, 1.0 - alpha], dtype=torch.float32))
+        self.ramp_dev.copy_(torch.tensor([thr, cw, 1.0 - alpha], dtype=torch.float32), non_blocking=True)
         return thr, cw, alpha
 
     def _finish(self, g, captured):
@@ -859,7 +865,7 @@ class DANStep(_TwoBatchStep):
         t = self.adam_t + 1
         b1, b2 = self.betas
         step_size, bc2_sqrt = self.disc_lr / (1 - b1 ** t), (1 - b2 ** t) ** 0.5          # as torch's Adam computes them (doubles)
-        self.ramp_dev.copy_(torch.tensor([cw, step_size, bc2_sqrt], dtype=torch.float32))
+        self.ramp_dev.copy_(torch.tensor([cw, step_size, bc2_sqrt], dtype=torch.float32), non_blocking=True)
         loss = self._run((image_l, label_l, image_u))
         self.adam_t = t
         self.parts = dict(self.parts, weight=cw)

@@ -12,7 +12,7 @@ from typing import NamedTuple
 import numpy as np
 import torch
 
-from ._lib import call
+from ._lib import LIB, call
 
 
 class SurfaceMetrics(NamedTuple):
@@ -89,8 +89,13 @@ def surface_metrics(pred, gt, classes, voxelspacing=None, workspace=None):
         out = torch.empty((classes - 1, 12), dtype=torch.float64, device=pred.device)
         call("wsl_surface_metrics", pred.contiguous(), gt.contiguous(), ndim, S, H, W, classes, sz, sy, sx, ws, out)
         o = out.cpu().numpy()
+    return decode(o)
+
+
+def decode(rows):
+    """[classes-1, 12] float64 rows of the metrics kernels (see include/wsl4mis_b200.h) -> [SurfaceMetrics] indexed by class - 1"""
     res = []
-    for r in o:
+    for r in rows:
         inter, npred, ngt, union, na, nb = (int(v) for v in r[:6])
         if npred and ngt:
             hd, asd = float(_percentile95(float(r[10]), float(r[11]), na + nb)), float(r[6] / na)
@@ -98,6 +103,64 @@ def surface_metrics(pred, gt, classes, voxelspacing=None, workspace=None):
             hd = asd = float("nan")
         res.append(SurfaceMetrics(inter, npred, ngt, union, hd, asd))
     return res
+
+
+_VOLUME = np.dtype([("voff", "<i8"), ("roff", "<i8"), ("coff", "<i8"), ("S", "<i4"), ("H", "<i4"), ("W", "<i4"), ("rank3", "<i4"),
+                    ("sz", "<f8"), ("sy", "<f8"), ("sx", "<f8")])
+
+
+class VolumeSet:
+    """A set of V label volumes of their own shapes ([S,H,W] or [H,W]) packed back to back, scored by ONE batched metrics launch
+    sequence (`wsl_surface_metrics_batched`) into [V, classes-1, 12] rows, bit-identical to V `surface_metrics` calls.  The volume
+    table and the workspace are allocated once, here, on `device`; `offsets[v]` is volume v's first voxel in the packed arrays."""
+
+    def __init__(self, shapes, classes, spacings=None, device="cuda"):
+        assert LIB.load().wsl_surface_metrics_volume_bytes() == _VOLUME.itemsize, "volume table layout mismatch"
+        self.shapes = [tuple(int(d) for d in s) for s in shapes]
+        self.classes, self.device = int(classes), torch.device(device)
+        if self.device.type == "cuda" and self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        V = len(self.shapes)
+        if V == 0:
+            raise ValueError("VolumeSet: no volumes")
+        tab = np.zeros(V, dtype=_VOLUME)
+        voff = roff = coff = 0
+        for v, shape in enumerate(self.shapes):
+            if len(shape) not in (2, 3):
+                raise ValueError(f"VolumeSet: volume {v} has rank {len(shape)} (2 or 3)")
+            S, H, W = ((1,) + shape) if len(shape) == 2 else shape
+            sp = _spacing(None if spacings is None else spacings[v], len(shape))
+            sz, sy, sx = ((1.0,) + sp) if len(shape) == 2 else sp
+            if not all(np.isfinite(x) and x > 0 for x in (sz, sy, sx)):
+                raise ValueError(f"VolumeSet: volume {v}: voxel spacing must be finite and > 0 (got {(sz, sy, sx)})")
+            surface_metrics_workspace_bytes(shape, classes)          # the single-volume limits hold for every volume
+            tab[v] = (voff, roff, coff, S, H, W, len(shape) == 3, sz, sy, sx)
+            voff, roff, coff = voff + S * H * W, roff + S * H, coff + H * W
+        self.offsets = [int(o) for o in tab["voff"]] + [voff]
+        self.n, self.rows, self.cols = voff, roff, coff
+        self.max_n = int(max(int(t["S"]) * int(t["H"]) * int(t["W"]) for t in tab))
+        self.max_w = int(tab["W"].max())
+        with torch.cuda.device(self.device):
+            self.table = torch.from_numpy(tab.view(np.uint8).copy()).to(self.device)
+            nbytes = ctypes.c_longlong(0)
+            call("wsl_surface_metrics_batched_workspace", V, self.n, self.rows, self.classes, ctypes.addressof(nbytes))
+            self.workspace = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
+
+    def __len__(self):
+        return len(self.shapes)
+
+    def __call__(self, pred, gt, out):
+        """enqueue the metrics of packed uint8 pred / gt ([n] CUDA) into out ([V, classes-1, 12] float64 CUDA); no host sync"""
+        V = len(self.shapes)
+        for name, t in (("pred", pred), ("gt", gt)):
+            if not (t.is_cuda and t.device == self.device and t.dtype == torch.uint8 and t.is_contiguous() and t.numel() == self.n):
+                raise ValueError(f"VolumeSet: {name} must be a contiguous uint8 tensor of {self.n} voxels on {self.device}")
+        if not (out.device == self.device and out.dtype == torch.float64 and tuple(out.shape) == (V, self.classes - 1, 12)):
+            raise ValueError(f"VolumeSet: out must be a float64 [{V}, {self.classes - 1}, 12] tensor on {self.device}")
+        with torch.cuda.device(self.device):
+            call("wsl_surface_metrics_batched", pred, gt, self.table, V, self.n, self.rows, self.cols, self.max_n, self.max_w,
+                 self.classes, self.workspace, out)
+        return out
 
 
 def _binary(result, reference, voxelspacing, connectivity):
