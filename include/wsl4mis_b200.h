@@ -436,6 +436,11 @@ int wsl_sgd_step(float* param, const float* grad, float* mom, long long n, const
  * Python scalars; scalars_ptr (device, {step_size, bc2_sqrt} in fp32) replaces the by-value pair so a captured graph follows t. */
 int wsl_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n, const float* scalars_ptr,
                   double step_size, double bc2_sqrt, double beta1, double beta2, double eps, cudaStream_t stream);
+/* wsl_adam_step on grad_scale * grad: the scale acts before the moments, so the data-parallel DAN step (engine.py DANStep._adam)
+ * runs Adam on the mean 1/world * (all-reduced sum of D's gradients).  wsl_adam_step is this entry at grad_scale 1 (same bits). */
+int wsl_adam_step_scaled(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n, const float* scalars_ptr,
+                         double step_size, double bc2_sqrt, double beta1, double beta2, double eps, double grad_scale,
+                         cudaStream_t stream);
 
 #ifdef __cplusplus
 }

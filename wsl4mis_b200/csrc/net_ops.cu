@@ -1432,14 +1432,15 @@ __global__ void __launch_bounds__(TPB) sgd_kernel(float* __restrict__ p, const f
 // torch.optim.Adam (weight_decay 0, amsgrad off), one step over a flat buffer, rounded where torch's multi-tensor path rounds:
 // each foreach op stores its result, and `a + s * b` compiles to one fma there as here.  w1 = 1 - beta1, w2 = 1 - beta2, eps and
 // the two t-dependent scalars are the fp32 values of torch's Python doubles; scal_ptr (device) = {lr / (1 - beta1^t),
-// sqrt(1 - beta2^t)} replaces the by-value pair so a captured CUDA graph follows t.
+// sqrt(1 - beta2^t)} replaces the by-value pair so a captured CUDA graph follows t.  gscale multiplies the gradient before the
+// moments (1/world turns an all-reduced sum into the mean; Adam is not scale-invariant because of eps); g * 1.0f is exact.
 __global__ void __launch_bounds__(TPB) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                    float* __restrict__ v, long long n, const float* scal_ptr, float step_size,
-                                                   float bc2_sqrt, float w1, float b2, float w2, float eps) {
+                                                   float bc2_sqrt, float w1, float b2, float w2, float eps, float gscale) {
   const float ss = scal_ptr ? scal_ptr[0] : step_size;
   const float bc = scal_ptr ? scal_ptr[1] : bc2_sqrt;
   for (long long i = blockIdx.x * (long long)TPB + threadIdx.x; i < n; i += (long long)gridDim.x * TPB) {
-    const float gi = g[i];
+    const float gi = g[i] * gscale;
     const float mi = fmaf(w1, gi - m[i], m[i]);             // exp_avg.lerp_(g, 1 - beta1): weight < 0.5 branch of at::lerp
     float vi = v[i] * b2;                                   // exp_avg_sq.mul_(beta2)
     vi = fmaf(w2, gi * gi, vi);                             //           .addcmul_(g, g, value=1 - beta2)
@@ -1852,13 +1853,19 @@ WSL_API int wsl_sgd_step(float* param, const float* grad, float* mom, long long 
   return wsl_check_launch("sgd_step");
 }
 
-WSL_API int wsl_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n, const float* scalars_ptr,
-                          double step_size, double bc2_sqrt, double beta1, double beta2, double eps, cudaStream_t stream) {
+WSL_API int wsl_adam_step_scaled(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
+                                 const float* scalars_ptr, double step_size, double bc2_sqrt, double beta1, double beta2, double eps,
+                                 double grad_scale, cudaStream_t stream) {
   WSL_REQUIRE(n >= 0 && beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "wsl_adam_step: bad betas (%g, %g)", beta1, beta2);
   if (n == 0) return 0;
   adam_kernel<<<grid_for(n), TPB, 0, stream>>>(param, grad, exp_avg, exp_avg_sq, n, scalars_ptr, (float)step_size, (float)bc2_sqrt,
-                                               (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps);
+                                               (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps, (float)grad_scale);
   return wsl_check_launch("adam_step");
+}
+
+WSL_API int wsl_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n, const float* scalars_ptr,
+                          double step_size, double bc2_sqrt, double beta1, double beta2, double eps, cudaStream_t stream) {
+  return wsl_adam_step_scaled(param, grad, exp_avg, exp_avg_sq, n, scalars_ptr, step_size, bc2_sqrt, beta1, beta2, eps, 1.0, stream);
 }
 
 WSL_API int wsl_conv_first(const float* x, const float* w, const float* bias, void* y, int dtype, int N, int H, int W, int Cout,

@@ -44,13 +44,15 @@ class RandomGenerator:
         self.output_size = tuple(int(v) for v in output_size)
 
     @staticmethod
-    def draw(label_has_4):
-        if random.random() > 0.5:
-            k = int(np.random.randint(0, 4))              # random_rot_flip, :126-134
-            axis = int(np.random.randint(0, 2))
+    def draw(label_has_4, streams=None):
+        """streams: (Python Random, numpy RandomState) to draw from instead of the global `random` / `np.random` (`rank_streams`)"""
+        py, npr = (random, np.random) if streams is None else streams
+        if py.random() > 0.5:
+            k = int(npr.randint(0, 4))                    # random_rot_flip, :126-134
+            axis = int(npr.randint(0, 2))
             return (1, k, axis, 0, 0)
-        elif random.random() > 0.5:
-            angle = int(np.random.randint(-20, 20))       # random_rotate, :137-143
+        elif py.random() > 0.5:
+            angle = int(npr.randint(-20, 20))             # random_rotate, :137-143
             return (2, 0, 0, angle, 4 if label_has_4 else 0)
         return (0, 0, 0, 0, 0)
 
@@ -62,6 +64,14 @@ class RandomGenerator:
         label = np.asarray(sample["label"]).astype(np.uint8)
         img, lab = apply_host(image, label, self.draw(bool((label == 4).any())), self.output_size)
         return {"image": torch.from_numpy(img).unsqueeze(0), "label": torch.from_numpy(lab)}
+
+
+def rank_streams(seed, rank):
+    """(random.Random, np.random.RandomState) of one data-parallel rank, seeded from (seed, rank): the ranks of one job draw
+    different augmentation parameters for their shards, while the global streams, which the steps' own host draws use, stay
+    identical on every rank"""
+    ss = np.random.SeedSequence([int(seed), int(rank)])
+    return random.Random(int(ss.generate_state(1, np.uint64)[0])), np.random.RandomState(ss.generate_state(4))
 
 
 def apply_host(image, label, params, output_size):
@@ -440,13 +450,16 @@ class GpuLoader:
     """Replaces ``DataLoader(db_train, batch_size, shuffle=True)`` + ``RandomGenerator`` for the training split: yields
     ``{'image': [B,1,H,W] fp32 cuda, 'label': [B,H,W] uint8 cuda, 'idx': [...]}`` (script keys, dataset_semi.py:120-124)."""
 
-    def __init__(self, store, batch_size, output_size=(256, 256), shuffle=True, drop_last=False, rank=0, world_size=1):
+    def __init__(self, store, batch_size, output_size=(256, 256), shuffle=True, drop_last=False, rank=0, world_size=1, streams=None):
         """`batch_size` is per rank.  With world_size > 1 every rank walks the SAME permutation (all ranks seed torch alike, as
-        the scripts do with args.seed) and takes the strided share rank::world_size of it, like DistributedSampler."""
+        the scripts do with args.seed) and takes the strided share rank::world_size of it, like DistributedSampler.  streams:
+        the (random.Random, np.random.RandomState) the augmentation parameters are drawn from (`rank_streams`); None: the global
+        `random` / `np.random`, as the scripts' transform draws."""
         self.store, self.batch_size, self.shuffle, self.drop_last = store, int(batch_size), shuffle, drop_last
         self.rank, self.world_size = int(rank), int(world_size)
         assert 0 <= self.rank < self.world_size
         self.transform = RandomGenerator(output_size)
+        self.streams = streams
 
     @staticmethod
     def shard(order, rank, world_size):
@@ -481,7 +494,7 @@ class GpuLoader:
 
     def __iter__(self):
         for idx in self._batches():
-            params = [self.transform.draw(bool(self.store.has4[i])) for i in idx]
+            params = [self.transform.draw(bool(self.store.has4[i]), self.streams) for i in idx]
             img, lab = self.store.augment(idx, params, self.transform.output_size)
             yield {"image": img, "label": lab, "idx": [self.store.names[i] for i in idx]}
 
@@ -494,11 +507,13 @@ class S2LLoader(GpuLoader):
     batches see the prediction memory as it was at that moment; the snapshot is taken when iteration starts and a refresh in
     mid-epoch reaches the batches of the next epoch.  visibility='live': batches read the memory the refresh updates."""
 
-    def __init__(self, store, batch_size, output_size=(256, 256), shuffle=True, drop_last=False, visibility="epoch"):
+    def __init__(self, store, batch_size, output_size=(256, 256), shuffle=True, drop_last=False, visibility="epoch", rank=0,
+                 world_size=1, streams=None):
+        """rank, world_size, streams: `GpuLoader`'s (the same `shard` partition of every epoch's permutation)"""
         assert store.scribbles is not None, "S2LLoader needs a SliceStore built with scribbles="
         if visibility not in ("epoch", "live"):
             raise ValueError(f"visibility must be 'epoch' or 'live' (got {visibility!r})")
-        super().__init__(store, batch_size, output_size, shuffle, drop_last)
+        super().__init__(store, batch_size, output_size, shuffle, drop_last, rank, world_size, streams)
         self.visibility = visibility
 
     def __iter__(self):
@@ -506,6 +521,6 @@ class S2LLoader(GpuLoader):
             self.store.weight_epoch.copy_(self.store.weight_live)
         for idx in self._batches():
             # the draws of RandomGenerator_s2l are RandomGenerator's; the scribble is rotated with cval 0 (SURVEY F15)
-            params = [self.transform.draw(False) for _ in idx]
+            params = [self.transform.draw(False, self.streams) for _ in idx]
             img, scr, wgt = self.store.augment_s2l(idx, params, self.transform.output_size, self.visibility)
             yield {"image": img, "scribble": scr, "weight": wgt, "idx": [self.store.names[i] for i in idx]}

@@ -71,6 +71,15 @@ def _masks(model):
     return getattr(model, "dropout_masks", None), getattr(model, "channel_keep", None)
 
 
+def _require_group(name, world_size, pg):
+    """world_size > 1 needs an initialised process group of that many ranks: without one the all-reduces would do nothing while
+    the optimisers still divide by world_size"""
+    import torch.distributed as dist
+    if int(world_size) > 1 and not (dist.is_available() and dist.is_initialized() and dist.get_world_size(pg) == int(world_size)):
+        raise NotImplementedError(f"{name}(world_size={world_size}) needs an initialised torch.distributed process group of "
+                                  f"{world_size} ranks; without one it runs on one GPU (world_size=1)")
+
+
 def _aux_ids(model):
     """ids of the aux decoder's parameters on a two-decoder model (unet_cct): steps that read main_seg only (SURVEY F7) skip them"""
     return {id(q) for q in model.aux_decoder1.parameters()} if len(model.executor.dec) == 2 else set()
@@ -199,13 +208,13 @@ class _FlatSGDStep:
                 k = (k, shapes)
             if k not in self._graphs:
                 self._graphs[k] = self._capture(inputs, kw) + (tuple(getattr(self, a) for a in self.aliases),)
-            g1, g2, gloss, gg, kept = self._graphs[k]
+            stages, gloss, kept = self._graphs[k]
             for a, v in zip(self.aliases, kept):
                 setattr(self, a, v)
-            g1.replay()
-            if g2 is not None:                  # two-graph mode: the all-reduce is issued from the host between the graphs
-                self._allreduce(gg)
-                g2.replay()
+            for graph, then in stages:          # several graphs: the all-reduces are issued from the host between them
+                graph.replay()
+                if then is not None:
+                    then()
             # the captured loss lives in graph-pool memory that the next replay overwrites: hand out a copy
             # (the aliased attributes, e.g. step.outputs, still point into the pool: read them before the next step)
             loss = gloss.clone()
@@ -213,28 +222,28 @@ class _FlatSGDStep:
         return loss
 
     def _capture(self, inputs, kw):
-        """Capture the step -> (graph, second graph or None, loss, gradient bucket).  world_size 1: one graph.  world_size > 1
-        with nccl_in_graph: ONE graph as well, with the all-reduces captured inside it (no host round trip and no second graph
-        launch between backward and optimiser); otherwise, or if this NCCL / torch build refuses to capture the collective, two
-        graphs (forward+backward | update) with the all-reduce issued from the host in between."""
+        """Capture the step -> (stages, loss): stages = [(graph, what the host runs after its replay, or None)].  world_size 1:
+        one graph.  world_size > 1 with nccl_in_graph: ONE graph as well, with the all-reduces captured inside it (no host round
+        trip and no second graph launch between backward and optimiser); otherwise, or if this NCCL / torch build refuses to
+        capture the collective, two graphs (forward+backward | update) with the all-reduce issued from the host in between."""
         torch.cuda.synchronize()
         if self.world_size > 1 and self.nccl_in_graph:
             try:
                 g1, (gloss, gg) = _captured(lambda: self._step(inputs, kw, True))
                 self.comm_mode = "captured in the step graph (decoder slice overlapped with the encoder backward)" if self.overlap_comm else "captured in the step graph"
-                return g1, None, gloss, gg
+                return [(g1, None)], gloss
             except Exception as e:                   # pragma: no cover - depends on the NCCL build
                 self.comm_mode = f"two graphs, host-issued all-reduce (capture failed: {type(e).__name__})"
                 torch.cuda.synchronize()
                 self.overlap_comm = False            # a host-issued collective cannot sit inside backward()
         if self.world_size == 1:
             g1, (gloss, gg) = _captured(lambda: self._step(inputs, kw, True))
-            return g1, None, gloss, gg
+            return [(g1, None)], gloss
         if not hasattr(self, "comm_mode"):
             self.comm_mode = "two graphs, host-issued all-reduce"
         g1, (gloss, gg) = _captured(lambda: self._fwd_bwd(*inputs, **kw))
         g2, _ = _captured(lambda: self._finish(gg, True))
-        return g1, g2, gloss, gg
+        return [(g1, lambda: self._allreduce(gg)), (g2, None)], gloss
 
     def input_buffers(self, idx=0, like=None):
         """The device buffers read by the graphs of input set `idx` (0 .. input_sets - 1), one per tensor the step takes."""
@@ -739,17 +748,20 @@ class S2LStep(TrainStep):
     terms, their u-label map and the combined logit gradient come from two kernels; thr_conf and the before/after-thr_iter switch
     live in device memory (`ctrl`), so graph=True captures one graph that serves the whole run.  SGD / poly LR as TrainStep.
 
-    Only single-output models run this script (softmax(model(img)), :228); multi-GPU Scribble2Label is not supported."""
+    Only single-output models run this script (softmax(model(img)), :228).  world_size > 1: batch-sharded data parallel as
+    `TrainStep` (one all-reduce of the bucket per step; the pCE and u-label CE normalisers are per rank), and `refresh` splits the
+    slices over the ranks and gathers the prediction memory on every rank."""
 
     def __init__(self, model, thr_iter=6000, thr_conf=0.8, base_lr=0.01, max_iterations=60000, momentum=0.9, weight_decay=1e-4,
                  graph=True, world_size=1, **kw):
-        if int(world_size) != 1:
-            raise NotImplementedError("Scribble2Label runs on one GPU (world_size must be 1)")
+        if kw.get("global_batch") and int(world_size) > 1:
+            raise NotImplementedError("global_batch semantics are not defined for the Scribble2Label step (run it with per-rank normalisers)")
+        _require_group("S2LStep", world_size, kw.get("process_group"))
         ex = model.executor
         if len(ex.dec) != 1 or any(ex.ds_heads) or not hasattr(ex, "enc_blocks"):
             raise ValueError("Scribble2Label needs a single-output U-Net (train_s2l.py:228 takes softmax(model(img)))")
         super().__init__(model, "pce", base_lr=base_lr, max_iterations=max_iterations, momentum=momentum, weight_decay=weight_decay,
-                         graph=graph, **kw)
+                         graph=graph, world_size=world_size, **kw)
         self.thr_iter, self.thr_conf = int(thr_iter), float(thr_conf)
         self.ctrl = torch.tensor([self.thr_conf, 0.0], dtype=torch.float32, device=self.dev)    # {thr_conf, w_u}
         self._w_u = 0.0
@@ -793,13 +805,20 @@ class S2LStep(TrainStep):
 
         Here `chunk` slices run as ONE per-sample-BatchNorm forward (exactly what `chunk` batch-1 training forwards compute, the
         running statistics updated in slice order across chunks); one kernel then does softmax at the back-zoom source pixel
-        and the EMA.  masks (tests): dropout keep masks {encoder block: uint8 [len(store), h, w, C]} for the whole pass."""
+        and the EMA.  masks (tests): dropout keep masks {encoder block: uint8 [len(store), h, w, C]} for the whole pass.
+
+        world_size > 1: rank r refreshes the contiguous slices `ddp.shard_range(len(store), r, world_size)` in chunks of its own,
+        then each owner broadcasts its slices' contiguous range of the memory, so every rank ends with the whole memory (the next
+        epoch's shard holds other slices).  Each slice's result depends on its own statistics only, so with the same weights and
+        dropout masks the memory is the one-process refresh's; the running statistics take the updates of the rank's own slices,
+        and the device-drawn dropout masks are the rank's own, as in its training steps."""
         assert store.weight_live is not None, "the store has no prediction memory (SliceStore.from_arrays(..., scribbles=))"
         self.model.train()
         n, dev = len(store), store.images.device
         a, b = float(alpha), float(1.0 - alpha)
-        for s in range(0, n, int(chunk)):
-            idx = list(range(s, min(n, s + int(chunk))))
+        lo, hi = (0, n) if self.world_size == 1 else ddp.shard_range(n, torch.distributed.get_rank(self.pg), self.world_size)
+        for s in range(lo, hi, int(chunk)):
+            idx = list(range(s, min(hi, s + int(chunk))))
             B = len(idx)
             tab = store.table(idx, [(0, 0, 0, 0, 0)] * B)          # mode 0: zoom(order 0) only (:223-224)
             img = torch.empty(B, 1, size, size, dtype=torch.float32, device=dev)
@@ -809,6 +828,14 @@ class S2LStep(TrainStep):
             outs, _ = self.ex.forward(img, True, False, mk, None, bn_per_sample=True)
             max_hw = int(max(int(store.shapes[i, 0]) * int(store.shapes[i, 1]) for i in idx))
             call("wsl_s2l_refresh", outs[0], tab, B, size, max_hw, a, b, store.weight_live)
+        if self.world_size > 1:
+            import torch.distributed as dist
+            ranks = None if self.pg is None else dist.get_process_group_ranks(self.pg)
+            for r in range(self.world_size):
+                rlo, rhi = ddp.shard_range(n, r, self.world_size)
+                if rhi > rlo:
+                    end = int(store.offs[rhi - 1]) + int(store.shapes[rhi - 1, 0]) * int(store.shapes[rhi - 1, 1])
+                    ddp.broadcast_flat(store.weight_live[int(store.offs[rlo]): end], r if ranks is None else ranks[r], self.pg)
 
 
 class DANStep(_TwoBatchStep):
@@ -826,22 +853,29 @@ class DANStep(_TwoBatchStep):
     (D's weights change only in the Adam step at the end), and a `load_state_dict` between steps is picked up.  graph=True captures
     the whole iteration as one CUDA graph per batch shape after two eager warm-up steps at that shape: the first batch, a full one
     with B_u == B_l, and after it an epoch's shorter last batches; the ramp weight and Adam's t-dependent scalars are written to `ramp_dev` before every step.  The modules' train() / eval() flags are not touched: each pass runs in the script's mode.
-    Test hooks: `model.dropout_masks` (phase 1) and `disc.channel_keep` (phase 2, [B_l + B_u, C] masks) as for the modules."""
+    Test hooks: `model.dropout_masks` (phase 1) and `disc.channel_keep` (phase 2, [B_l + B_u, C] masks) as for the modules.
+
+    world_size > 1: batch-sharded data parallel with per-rank BatchNorm and loss normalisers, as the other two-batch steps.  The
+    student and D are broadcast from rank 0 at construction.  Phase 1's bucket is all-reduced (sum) and SGD applies the 1/world mean;
+    phase 2's D bucket is all-reduced (sum) and Adam runs on 1/world times it (`wsl_adam_step_scaled`: the scale acts before the
+    moments).  graph=True then captures three graphs per batch shape, phase 1 | SGD + phase 2 | Adam, with the two all-reduces issued
+    from the host between them."""
     scratch = "dan"
 
     def __init__(self, model, disc, base_lr=0.01, max_iterations=30000, consistency=0.1, consistency_rampup=200.0, disc_lr=1e-4,
-                 betas=(0.9, 0.99), graph=True, world_size=1):
-        if int(world_size) != 1:
-            raise NotImplementedError("DANStep runs on one GPU (world_size must be 1): the adversarial script has no multi-GPU form")
+                 betas=(0.9, 0.99), graph=True, world_size=1, process_group=None):
+        _require_group("DANStep", world_size, process_group)
         ex = model.executor
         if len(getattr(ex, "dec", ())) != 1 or any(getattr(ex, "ds_heads", ())):
             raise ValueError("DANStep needs a single-output segmentation network: the script takes torch.softmax(model(x), dim=1) "
                              "(train_deep_adversarial_network_2D.py:143-144), which fails on a tuple of outputs")
-        super().__init__(model, base_lr, max_iterations, consistency, consistency_rampup, 0.9, 1e-4, graph, 1, None)
+        super().__init__(model, base_lr, max_iterations, consistency, consistency_rampup, 0.9, 1e-4, graph, world_size, process_group)
         self.disc, self.dex = disc, disc.executor
         if next(disc.parameters()).device != self.dev:
             raise ValueError(f"DANStep: the discriminator is on {next(disc.parameters()).device}, the model on {self.dev}")
         self.dflat, self.doffsets = _flatten(list(disc.parameters()), self.dev)
+        if self.world_size > 1:
+            ddp.broadcast_flat(self.dflat, 0, self.pg)     # D's replicas start identical, as the student's
         self.dgrad = torch.zeros_like(self.dflat)
         self.exp_avg, self.exp_avg_sq = torch.zeros_like(self.dflat), torch.zeros_like(self.dflat)
         self.adam_t = 0
@@ -895,7 +929,30 @@ class DANStep(_TwoBatchStep):
         return {"loss_ce": ce, "loss_dice": dice, "consistency": term}
 
     def _finish(self, g, captured):
-        """student SGD (:158-160), then phase 2 (:162-178) and D's Adam step; host scalars come from ramp_dev in both modes"""
+        """student SGD (:158-160), then phase 2 (:162-178), the all-reduce of D's bucket and D's Adam step; host scalars come from
+        ramp_dev in both modes"""
+        self._phase2(g)
+        self._allreduce_disc()
+        self._adam()
+
+    def _allreduce_disc(self):
+        """sum D's gradient bucket over the ranks (the Adam step applies the 1/world mean)"""
+        if self.world_size > 1:
+            ddp.allreduce_flat(self.dgrad, self.pg)
+
+    def _capture(self, inputs, kw):
+        """world_size > 1: phase 1 | SGD + phase 2 | Adam as three graphs, with the student's and D's all-reduces between them"""
+        if self.world_size == 1:
+            return super()._capture(inputs, kw)
+        torch.cuda.synchronize()
+        self.comm_mode = "three graphs, host-issued all-reduces"
+        g1, (gloss, gg) = _captured(lambda: self._fwd_bwd(*inputs, **kw))
+        g2, _ = _captured(lambda: self._phase2(gg))
+        g3, _ = _captured(self._adam)
+        return [(g1, lambda: self._allreduce(gg)), (g2, self._allreduce_disc), (g3, None)], gloss
+
+    def _phase2(self, g):
+        """student SGD, then phase 2: D's loss and its gradient bucket `dgrad` on the updated student's eval-mode maps"""
         self._opt(g)
         ex, dex = self.ex, self.dex
         image_l, image_u = self._inputs
@@ -910,7 +967,13 @@ class DANStep(_TwoBatchStep):
         dloss, dlg = self._buf("disc_loss", (1,)), self._buf("dlogits_d", (N, 2))
         call("wsl_disc_ce", logits, N, B, None, 1.0, dloss, dlg)
         dex.backward(rec, dlg, False, False, bucket=(self.dgrad, self.doffsets))
-        b1, b2 = self.betas
-        call("wsl_adam_step", self.dflat, self.dgrad, self.exp_avg, self.exp_avg_sq, self.dflat.numel(), self.ramp_dev[1:3], 0.0, 0.0,
-             b1, b2, self.eps)
         self.parts["disc_loss"] = dloss[0]
+
+    def _adam(self):
+        b1, b2 = self.betas
+        if self.world_size == 1:
+            call("wsl_adam_step", self.dflat, self.dgrad, self.exp_avg, self.exp_avg_sq, self.dflat.numel(), self.ramp_dev[1:3], 0.0,
+                 0.0, b1, b2, self.eps)
+        else:
+            call("wsl_adam_step_scaled", self.dflat, self.dgrad, self.exp_avg, self.exp_avg_sq, self.dflat.numel(), self.ramp_dev[1:3],
+                 0.0, 0.0, b1, b2, self.eps, 1.0 / self.world_size)

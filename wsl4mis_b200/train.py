@@ -11,6 +11,13 @@ best-model saves on a strict improvement, ``iter_{N}.pth`` every 3000, the stop 
 scripts' logging format under ``../model/{exp}_{fold}/{sup_type}``.  ``--precision`` (bf16 | fp16 | fp16x3 | fp32, default bf16)
 is the one flag the scripts lack; graph capture is always on.
 
+Several GPUs: ``torchrun --nproc_per_node W -m wsl4mis_b200.train train_X.py ARGS`` runs W ranks, batch-sharded data parallel
+with per-rank BatchNorm statistics and loss normalisers (DESIGN §7).  ``--batch_size`` stays the script's global batch: each rank
+takes batch_size / W (the two-stream scripts batch_size / 2 / W per stream), and its loaders walk their `shard` of every epoch's
+permutation with augmentation draws from a stream of their own (`rank_streams`).  Rank 0 alone writes log.txt, TensorBoard scalars
+and checkpoints, validates, and logs its own shard's loss parts; the other ranks go on to the next step and meet it at that step's
+all-reduce.  With WORLD_SIZE unset or 1 nothing of this runs.
+
 Between two validation points the loop does not wait on the device: each iteration's loss parts are copied, in stream order,
 into a device buffer of up to 200 rows, and the buffer comes back in one device-to-host copy at each validation point, checkpoint
 and at the end; its lines are then written in iteration order ahead of what follows them, so ``log.txt`` has the script's lines in
@@ -50,7 +57,7 @@ def _flags(base, extra=(), **defaults):
 
 
 # One recipe per script.  kind: 'single' (GpuLoader), 's2l' (S2LLoader + ensemble refresh), 'semi' (zip(cycle(labelled), unlabelled)).
-# step: (args, model) -> step.  log: the per-iteration line (None: the script logs none), fed by iter_num, the loss and `cols`.
+# step: (args, model, world_size) -> step.  log: the per-iteration line (None: the script logs none), fed by iter_num, the loss and `cols`.
 # cols: (TensorBoard tag, step -> 0-dim device tensor) of the values after the loss; host: (tag, step -> float) values from the host.
 Recipe = namedtuple("Recipe", "flags kind step log cols host", defaults=((),))
 _LOG2 = 'iteration %d : loss : %f, loss_ce: %f'
@@ -62,9 +69,9 @@ def _part(name, attr="loss_parts"):
 
 
 def _train_step(variant):
-    def make(args, model):
+    def make(args, model, world_size=1):
         from .engine import TrainStep
-        step = TrainStep(model, variant, base_lr=args.base_lr, max_iterations=args.max_iterations, graph=True)
+        step = TrainStep(model, variant, base_lr=args.base_lr, max_iterations=args.max_iterations, graph=True, world_size=world_size)
         if variant == "pce_variance":
             step.consistency, step.consistency_rampup = args.consistency, args.consistency_rampup
         return step
@@ -72,7 +79,7 @@ def _train_step(variant):
 
 
 def _teacher_step(cls):
-    def make(args, model):
+    def make(args, model, world_size=1):
         from . import engine
         from .networks.net_factory import net_factory
         ema = net_factory(net_type=args.model, in_chns=1, class_num=args.num_classes)     # create_model(ema=True)
@@ -81,28 +88,29 @@ def _teacher_step(cls):
         ema.set_precision(model.precision)
         return getattr(engine, cls)(model, ema, base_lr=args.base_lr, max_iterations=args.max_iterations,
                                     **({} if cls == "USTMStep" else dict(consistency=args.consistency,
-                                                                          consistency_rampup=args.consistency_rampup)), graph=True)
+                                                                          consistency_rampup=args.consistency_rampup)), graph=True,
+                                    world_size=world_size)
     return make
 
 
-def _em_step(args, model):
+def _em_step(args, model, world_size=1):
     from .engine import EntropyMinStep
     return EntropyMinStep(model, base_lr=args.base_lr, max_iterations=args.max_iterations, consistency=args.consistency,
-                          consistency_rampup=args.consistency_rampup, graph=True)
+                          consistency_rampup=args.consistency_rampup, graph=True, world_size=world_size)
 
 
-def _dan_step(args, model):
+def _dan_step(args, model, world_size=1):
     from .engine import DANStep
     from .networks.discriminator import FCDiscriminator
     disc = FCDiscriminator(num_classes=args.num_classes).cuda()
     return DANStep(model, disc, base_lr=args.base_lr, max_iterations=args.max_iterations, consistency=args.consistency,
-                   consistency_rampup=args.consistency_rampup, graph=True)
+                   consistency_rampup=args.consistency_rampup, graph=True, world_size=world_size)
 
 
-def _s2l_step(args, model):
+def _s2l_step(args, model, world_size=1):
     from .engine import S2LStep
     return S2LStep(model, thr_iter=args.thr_iter, thr_conf=args.thr_conf, base_lr=args.base_lr, max_iterations=args.max_iterations,
-                   graph=True)
+                   graph=True, world_size=world_size)
 
 
 _CE = (("info/loss_ce", _part("ce")),)
@@ -185,6 +193,19 @@ def parse(argv):
     return script, parser_for(script).parse_args(rest), opts.precision
 
 
+def rank_batch(script, batch_size, world_size):
+    """the per-rank batch of a recipe: batch_size / W (the two-stream recipes: batch_size / 2 / W per stream); raises ValueError
+    when W > 1 does not divide it.  W = 1: the script's own batch_size (batch_size // 2 per stream)."""
+    per_stream = recipe_for(script).kind == "semi"
+    if world_size == 1:
+        return batch_size // 2 if per_stream else batch_size
+    div = 2 * world_size if per_stream else world_size
+    if batch_size % div:
+        raise ValueError(f"--batch_size {batch_size} does not split over {world_size} ranks: {os.path.basename(script)} needs a "
+                         f"multiple of {div}" + (" (two streams of batch_size / 2, each split over the ranks)" if per_stream else ""))
+    return batch_size // div
+
+
 def snapshot_path(args):
     return "../model/{}_{}/{}".format(args.exp, args.fold, args.sup_type)
 
@@ -235,8 +256,11 @@ class Trainer:
     ``score(model, classes)``; `log` takes one line; `writer` (optional) takes ``add_scalar(tag, value, step)``."""
 
     def __init__(self, args, recipe, model, step, batches, n_per_epoch, validator, snapshot, log, writer=None, refresh=None,
-                 device=None):
+                 device=None, rank=0):
+        """rank > 0: a data-parallel rank other than rank 0; it runs the steps (and the refresh) only, and never logs, validates or
+        saves"""
         self.args, self.recipe, self.model, self.step = args, recipe, model, step
+        self.main = int(rank) == 0
         self.batches, self.n_per_epoch, self.validator = batches, int(n_per_epoch), validator
         self.snapshot, self.log, self.writer, self.refresh = snapshot, log, writer, refresh
         dev = device if device is not None else next(model.parameters()).device
@@ -289,8 +313,9 @@ class Trainer:
         return best
 
     def run(self):
-        args, r, step = self.args, self.recipe, self.step
-        self.log("{} iterations per epoch".format(self.n_per_epoch))
+        args, r, step, main = self.args, self.recipe, self.step, self.main
+        if main:
+            self.log("{} iterations per epoch".format(self.n_per_epoch))
         iter_num, best = 0, 0.0
         max_epoch = args.max_iterations // self.n_per_epoch + 1
         for _ in range(max_epoch):
@@ -298,26 +323,30 @@ class Trainer:
                 lr = args.base_lr * (1.0 - iter_num / args.max_iterations) ** 0.9
                 loss = step(*inputs)
                 iter_num += 1
-                self.buffer.add(iter_num, lr, [loss] + [get(step) for _, get in r.cols], [get(step) for _, get in r.host])
-                if iter_num > 0 and iter_num % VAL_EVERY == 0:
+                if main:
+                    self.buffer.add(iter_num, lr, [loss] + [get(step) for _, get in r.cols], [get(step) for _, get in r.host])
+                if main and iter_num > 0 and iter_num % VAL_EVERY == 0:
                     self._flush()
                     best = self._validate(iter_num, best)
-                if iter_num % SAVE_EVERY == 0:
+                if main and iter_num % SAVE_EVERY == 0:
                     self._flush()
                     path = os.path.join(self.snapshot, 'iter_' + str(iter_num) + '.pth')
                     self._save([path])
                     self.log("save model to {}".format(path))
                 if self.refresh is not None and iter_num > 0 and iter_num % args.period_iter == 0:
-                    if r.log is not None:
+                    if main and r.log is not None:
                         self._flush()
-                    self.log("update weight start")
-                    self.refresh()
-                    self.log("update weight end")
+                    if main:
+                        self.log("update weight start")
+                    self.refresh()          # every rank: the refresh is split over the ranks and gathered on all of them
+                    if main:
+                        self.log("update weight end")
                 if iter_num >= args.max_iterations:
                     break
             if iter_num >= args.max_iterations:
                 break
-        self._flush()
+        if main:
+            self._flush()
         return "Training Finished!"
 
 
@@ -341,12 +370,14 @@ def two_stream(loader_l, loader_u, labelled_only=False):
         yield (bl["image"], bl["label"]) if labelled_only else (bl["image"], bl["label"], bu["image"])
 
 
-def build(script, args, precision):
+def build(script, args, precision, rank=0, world_size=1):
     """-> (model, step, batches, iterations per epoch, refresh or None): the recipe's network, step and loaders, seeded as the
-    script seeds them (random / numpy / torch with --seed, then net_factory)"""
-    from .dataloaders.dataset import BaseDataSets, BaseDataSets_s2l, GpuLoader, S2LLoader
+    script seeds them (random / numpy / torch with --seed, then net_factory).  world_size > 1: rank `rank`'s step, and its loaders
+    over its shard of each epoch at `rank_batch`, drawing their augmentation parameters from `rank_streams(--seed, rank)`."""
+    from .dataloaders.dataset import BaseDataSets, BaseDataSets_s2l, GpuLoader, S2LLoader, rank_streams
     from .networks.net_factory import net_factory
     recipe = recipe_for(script)
+    bs = rank_batch(script, args.batch_size, world_size)
     random.seed(args.seed)
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
@@ -356,36 +387,60 @@ def build(script, args, precision):
         raise ValueError(f"net_factory does not build --model {args.model!r}")
     model.set_precision(precision)
     size = tuple(int(x) for x in args.patch_size)
+    shard = dict(rank=rank, world_size=world_size, streams=rank_streams(args.seed, rank) if world_size > 1 else None)
     refresh = None
     if recipe.kind == "semi":
         from .dataloaders.dataset_semi import BaseDataSets as SemiSets
         store_l = SemiSets(base_dir=args.root_path, labeled_type="labeled", fold=args.fold, split="train").to_slice_store()
         store_u = SemiSets(base_dir=args.root_path, labeled_type="unlabeled", fold=args.fold, split="train").to_slice_store()
-        loader_l, loader_u = GpuLoader(store_l, args.batch_size // 2, size), GpuLoader(store_u, args.batch_size // 2, size)
-        step = recipe.step(args, model)
+        loader_l, loader_u = GpuLoader(store_l, bs, size, **shard), GpuLoader(store_u, bs, size, **shard)
+        step = recipe.step(args, model, world_size)
         labelled_only = script == "train_partially_fully_supervised.py"
         batches = lambda: two_stream(loader_l, loader_u, labelled_only)
         n = len(loader_l)
     elif recipe.kind == "s2l":
         store = BaseDataSets_s2l(base_dir=args.root_path, fold=args.fold).to_slice_store()
-        loader = S2LLoader(store, args.batch_size, size)
-        step = recipe.step(args, model)
+        loader = S2LLoader(store, bs, size, **shard)
+        step = recipe.step(args, model, world_size)
         batches = lambda: ((b["image"], b["scribble"], b["weight"]) for b in loader)
         n = len(loader)
         refresh = lambda: step.refresh(store, alpha=args.alpha)
     else:
         store = BaseDataSets(base_dir=args.root_path, split="train", fold=args.fold, sup_type=args.sup_type).to_slice_store()
-        loader = GpuLoader(store, args.batch_size, size)
-        step = recipe.step(args, model)
+        loader = GpuLoader(store, bs, size, **shard)
+        step = recipe.step(args, model, world_size)
         batches = lambda: ((b["image"], b["label"]) for b in loader)
         n = len(loader)
     return model, step, batches, n, refresh
 
 
 def train(argv):
-    """run one recipe from its command line ([script, flags...]); -> the snapshot directory"""
-    from .val_2D import ValidationSet
+    """run one recipe from its command line ([script, flags...]); -> the snapshot directory.  Under torchrun (WORLD_SIZE > 1)
+    each process is one rank on cuda:LOCAL_RANK, in an NCCL process group it creates and destroys (a caller that already holds
+    one keeps it)."""
+    import torch.distributed as dist
+    from .ddp import env_world
     script, args, precision = parse(argv)
+    rank, local_rank, world = env_world()
+    rank_batch(script, args.batch_size, world)          # a batch that does not split raises before anything is built
+    own_group = world > 1 and not dist.is_initialized()
+    if own_group:
+        torch.cuda.set_device(local_rank)
+        dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
+    try:
+        if rank == 0:
+            return _train_logged(script, args, precision, world)
+        model, step, batches, n, refresh = build(script, args, precision, rank, world)
+        Trainer(args, recipe_for(script), model, step, batches, n, None, None, lambda msg: None, None, refresh, rank=rank).run()
+        return snapshot_path(args)
+    finally:
+        if own_group:
+            dist.destroy_process_group()
+
+
+def _train_logged(script, args, precision, world=1):
+    """rank 0 (or the one process): log.txt, TensorBoard, validation and checkpoints around the loop"""
+    from .val_2D import ValidationSet
     snapshot = snapshot_path(args)
     os.makedirs(snapshot, exist_ok=True)
     logger = logging.getLogger("wsl4mis_b200.train")
@@ -399,7 +454,7 @@ def train(argv):
     writer = None
     try:
         logger.info(str(args))
-        model, step, batches, n, refresh = build(script, args, precision)
+        model, step, batches, n, refresh = build(script, args, precision, 0, world)
         val_fold = "fold1" if script in VAL_FOLD_DEFAULT else args.fold
         validator = ValidationSet(args.root_path, fold=val_fold)
         writer = _summary_writer(snapshot + '/log')
