@@ -238,6 +238,7 @@ int wsl_surface_metrics_batched(const uint8_t* pred, const uint8_t* gt, const vo
 /* nn.Conv2d(k=3,pad=1)/(k=1) forward on CUDA cores (unet.py:19,23,55,120); with dgrad-packed weights also the
  * data gradient.  Two channels-last sources model torch.cat([x2,x1],1) (unet.py:67).
  * out_mode 0: bf16 NHWC with CoutStore channels; 1: fp32 NCHW with CoutStore channels; 2: fp32 NHWC; 3: fp16 NHWC.
+ * The 16-bit modes 0 and 3 need CoutStore % 8 == 0 (returns -1 otherwise).
  * src_f32 (a dtype code): 1 = sources are fp32 (a single-channel image, or fp32 NHWC activations with C %% 8 == 0),
  * 0 = bf16, 2 = fp16; likewise dy_f32 of the weight gradient. */
 int wsl_conv_direct(const void* src0, int C0, const void* src1, int C1, int src_f32, const float* wpk,

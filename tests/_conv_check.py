@@ -9,8 +9,13 @@ fp32 accumulation noise.  A missing tap, k-block or
 tile is about S / (taps * k-blocks), far above the slack, and the bound is per element, so one wrong 8 x 16 tile cannot hide
 under the tensor's maximum.  NaN (an output never written) always fails.
 
+The CUDA-core direct convolution (conv_direct_kernel: the fp32 mode's forward and data gradient) sums K = taps * Cin products
+with K sequential fp32 FMAs in a fixed order; see direct_slack for its allowance.  Its fp32 outputs use u = 2^-24 for the final
+bias addition (direct_u).
+
 Weight gradients.  rel-L2 against fp64 <= 1e-4, per (output-channel block, input-channel block), i.e. per output tile of the
-split-K kernels: leaving out one 128-pixel chunk of P pixels moves a tile by about sqrt(128 / P)."""
+split-K kernels: leaving out one 128-pixel chunk of P pixels moves a tile by about sqrt(128 / P).  Bias gradients (per-channel sums)
+within STAT_TOL of the summed magnitudes (check_sums)."""
 import math
 
 import torch
@@ -19,7 +24,26 @@ import torch.nn.functional as F
 SLACK_16 = 2.0 ** -16       # 16-bit operands, fp32 accumulation
 UNIT_ROUNDOFF = {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11, torch.float32: 0.0}
 WGRAD_TOL = 1e-4
+STAT_TOL = 1e-5             # per-channel sums against fp64, relative to the sum of the magnitudes
 CHUNK_PX = 128              # pixels per split-K chunk of every weight-gradient kernel (16 x 8 or 8 x 16)
+
+
+def direct_slack(K):
+    """Accumulation allowance (times S) of the direct convolution with K = taps * Cin terms per output.  Each FMA rounds its partial
+    sum once, by at most 2^-24 of a partial sum that never exceeds S.  Round-to-nearest errors are uncorrelated, so they add like a
+    random walk: in the worst case for the noise, same-signed terms whose partial sums grow linearly to S, the standard deviation of
+    the sum is 2^-24 S sqrt(sum_k (k / K)^2 / 3) = sqrt(K) / 3 * 2^-24 S.  The allowance is 2 sqrt(K) 2^-24 (six of those standard
+    deviations) and never below 2^-20, which bounds the K <= 15 roundings of the single-channel image layer outright.  With
+    zero-mean operands the partial sums random-walk far below S and the noise stays a few 2^-24 S at any K.  At the deepest layer
+    (the discriminator's last, K = 9 * 1024) the allowance is 1.1e-5 S, a tenth of one average term S / K: a dropped tap, channel
+    or 16-channel chunk is far above it."""
+    return max(2.0 ** -20, 2.0 * math.sqrt(K) * 2.0 ** -24)
+
+
+def direct_u(dtype):
+    """rounding allowance relative to |ref| of a direct-convolution output stored as `dtype`: the 16-bit store, or for fp32 the
+    final bias addition"""
+    return UNIT_ROUNDOFF[dtype] if dtype != torch.float32 else 2.0 ** -24
 
 
 def split_slack(K):
@@ -141,3 +165,12 @@ def check_wgrad(got, ref, co_blk, ci_blk, tol=WGRAD_TOL):
             worst = max(worst, e / tol if e == e else math.inf)
     rel = ((got - ref).norm() / ref.norm().clamp_min(1e-300)).item()
     return {"worst": worst, "bad": bad, "rel": rel}
+
+
+def check_sums(got, ref, mag, tol=STAT_TOL):
+    """per-channel sums (a bias gradient) against fp64: |got - ref| <= tol * mag, mag = the sum of the magnitudes of the terms.
+    Returns {'worst': max error / bound, 'bad': [channels over the bound]}."""
+    err = (got.double() - ref.double()).abs()
+    bound = tol * mag.double()
+    ratio = torch.where(err == err, err / bound.clamp_min(1e-300), torch.full_like(err, math.inf))
+    return {"worst": ratio.max().item(), "bad": (~(err <= bound)).nonzero().flatten().tolist()}

@@ -1,5 +1,5 @@
-"""Every tensor-core convolution launch of a training step, replayed at the step's own batch sizes and checked per element
-against fp64 (tests/_conv_check.py states the bounds).
+"""Every convolution launch of a training step and of the evaluation forwards (tensor-core and CUDA-core kernels), replayed at the
+steps' own batch sizes and checked per element against fp64 (tests/_conv_check.py states the bounds).
 
 The launches are not hand-written: one eager forward + backward of the model runs with a recorder in place of
 wsl4mis_b200._lib.PROFILE, which keeps each distinct (entry point, scalar arguments, NULL pointer arguments) of the
@@ -9,11 +9,23 @@ shapes: 16-bit-rounded inputs whose channels carry scales from 2^-4 .. 2^4 (a mi
 tiles or row items, so the mbarrier phase carried across tiles, the per-tile accumulator reset, the BatchNorm partial sums over a
 CTA's tiles and the split-K chunk loops all run; the coverage test asserts that from the device's SM count.
 
+The configurations are the recipes' batches (6, 12, 16, 24 and bench.py's 64) in training (forward + backward), the evaluation
+forwards of the resident validation pass (64 slices), of the test step (16) and of the adversarial step's maps (6), the fp32 mode
+(which runs every layer on the CUDA-core wsl_conv_direct / wsl_wgrad_direct) and the discriminator of the adversarial step.  A
+distinct launch is replayed once however many configurations make it.  The census test runs one eager iteration of every recipe in
+wsl4mis_b200.train.RECIPES, one validation pass and one test-step volume, and requires every convolution launch they make to be
+among the replayed ones.
+
 Per launch: outputs within |got - ref| <= u |ref| + slack S; fused BatchNorm rows equal the fp64 sums of the stored outputs and
 wsl_bn_finalize turns them into fp64-accurate mean / invstd; weight gradients within rel-L2 1e-4 per output tile, bit-identical
-on the deterministic split-K path, within the same bound on the atomics path, and accumulating (a second call adds on top)."""
+on the deterministic split-K path, within the same bound on the atomics path, and accumulating (a second call adds on top).
+The direct convolution's replay takes any recorded form: one or two sources of any storage type (the single-channel fp32 image
+included), ksize 1 or 3, every out_mode, a forward with bias or a data gradient through the 'wd' pack; its weight gradient is
+checked with dbias against the fp64 sums of dY."""
 import ctypes
+import gc
 import math
+import time
 import zlib
 
 import pytest
@@ -28,46 +40,93 @@ DEV = "cuda"
 if torch.cuda.is_available():
     from wsl4mis_b200 import _lib
     from wsl4mis_b200._lib import call
+    from wsl4mis_b200.networks.discriminator import FCDiscriminator
     from wsl4mis_b200.networks.pnet import PNet2D
-    from wsl4mis_b200.networks.unet import UNet_CCT
+    from wsl4mis_b200.networks.unet import UNet, UNet_CCT
 
 CONV = ("wsl_conv_tc", "wsl_conv_tc_dil", "wsl_conv_tc2", "wsl_conv_tc_split")
 WGRAD = ("wsl_wgrad_tc", "wsl_wgrad_tc2", "wsl_wgrad_tc3", "wsl_wgrad_tc_dil", "wsl_wgrad_tc_split")
-HARVESTED = CONV + WGRAD + ("wsl_split_f32",)
+DIRECT = ("wsl_conv_direct", "wsl_wgrad_direct")
+HARVESTED = CONV + WGRAD + DIRECT + ("wsl_split_f32",)
 T16 = {0: torch.bfloat16, 2: torch.float16}
+DTYPE = {0: torch.bfloat16, 1: torch.float32, 2: torch.float16}              # dtype codes of the C ABI
+DTN = {0: "bf16", 1: "fp32", 2: "fp16"}
+OUT_T = {0: torch.bfloat16, 1: torch.float32, 2: torch.float32, 3: torch.float16}   # out_mode -> stored type
 REF_BYTES = 2 << 30          # fp64 reference working set per image chunk
-STAT_TOL = 1e-5              # BatchNorm rows vs fp64 sums, relative to sum |y| and sum y^2
+STAT_TOL = CC.STAT_TOL       # BatchNorm rows vs fp64 sums, relative to sum |y| and sum y^2
+DBIAS_MARGIN = 10            # a direct weight gradient's smallest split share of dbias, in units of its bound
 
-# (model, N, precision): N = 12 is the scripts' training batch, N = 64 bench.py's
+# (model, N, precision, mode): mode 'train' = forward + backward, 'eval' = eval-mode forward under no_grad.  N = 12 is the scripts'
+# training batch, 6 / 16 / 24 the other recipes' (and each semi-supervised stream's), 64 bench.py's and the validation chunk, 16 the
+# test step's chunk, 6 the adversarial step's no-grad maps of the unlabelled batch; the discriminator runs at that step's B = 6 and
+# 2B = 12.
 CONFIGS = {
-    "unet_cct-n12-bf16": ("unet_cct", 12, "bf16"),
-    "unet_cct-n64-bf16": ("unet_cct", 64, "bf16"),
-    "unet_cct-n12-fp16": ("unet_cct", 12, "fp16"),
-    "unet_cct-n12-fp16x3": ("unet_cct", 12, "fp16x3"),
-    "pnet2d-n12-bf16": ("pnet2d", 12, "bf16"),
+    "unet_cct-n12-bf16": ("unet_cct", 12, "bf16", "train"),
+    "unet_cct-n64-bf16": ("unet_cct", 64, "bf16", "train"),
+    "unet_cct-n12-fp16": ("unet_cct", 12, "fp16", "train"),
+    "unet_cct-n12-fp16x3": ("unet_cct", 12, "fp16x3", "train"),
+    "pnet2d-n12-bf16": ("pnet2d", 12, "bf16", "train"),
+    "pnet2d-n12-fp16": ("pnet2d", 12, "fp16", "train"),
+    "unet_cct-n12-fp32": ("unet_cct", 12, "fp32", "train"),
+    "unet_cct-n64-fp32": ("unet_cct", 64, "fp32", "train"),
+    "unet-n64-bf16-eval": ("unet", 64, "bf16", "eval"),
+    "unet-n16-bf16-eval": ("unet", 16, "bf16", "eval"),
+    "unet-n6-bf16-eval": ("unet", 6, "bf16", "eval"),
+    "unet_cct-n6-bf16": ("unet_cct", 6, "bf16", "train"),
+    "unet_cct-n16-bf16": ("unet_cct", 16, "bf16", "train"),
+    "unet_cct-n24-bf16": ("unet_cct", 24, "bf16", "train"),
+    "disc-n6-bf16": ("disc", 6, "bf16", "train"),
+    "disc-n12-bf16": ("disc", 12, "bf16", "train"),
 }
-_RESULTS = {}
+_RESULTS, _REPLAYS, _KEYS = {}, {}, {}
 
 
-def _harvest(model, N, precision):
-    torch.manual_seed(0)
-    m = UNet_CCT(1, 4) if model == "unet_cct" else PNet2D(1, 4, 64, [1, 2, 4, 8, 16])
-    m = m.to(DEV).set_precision(precision)
-    m.train()
-    x = torch.rand(N, 1, 256, 256, device=DEV)
+def _model(kind):
+    if kind == "unet_cct":
+        return UNet_CCT(1, 4)
+    if kind == "unet":
+        return UNet(1, 4)
+    if kind == "disc":
+        return FCDiscriminator(4)
+    return PNet2D(1, 4, 64, [1, 2, 4, 8, 16])
+
+
+def _record(run):
+    """the distinct convolution launches of run()"""
     rec, saved = LaunchRecorder(lambda name: name in HARVESTED), _lib.PROFILE
     _lib.PROFILE = rec
     try:
-        out = m(x)
-        outs = out if isinstance(out, (tuple, list)) else (out,)
-        loss = sum((o.float() * torch.randn_like(o.float())).mean() for o in outs)
-        loss.backward()
+        run()
         torch.cuda.synchronize()
     finally:
         _lib.PROFILE = saved
-    del m, out, outs, loss
+    gc.collect()
     torch.cuda.empty_cache()
     return rec.launches
+
+
+def _harvest(model, N, precision, mode):
+    torch.manual_seed(0)
+    m = _model(model).to(DEV).set_precision(precision)
+    x = torch.rand(N, 1, 256, 256, device=DEV)
+
+    def run():
+        if mode == "eval":
+            m.eval()
+            with torch.no_grad():
+                m(x)
+            return
+        m.train()
+        if model == "disc":           # the adversarial step back-propagates into the segmentation maps
+            mp = torch.softmax(torch.randn(N, 4, 256, 256, device=DEV), 1).requires_grad_(True)
+            out = m(mp, x)
+        else:
+            out = m(x)
+        outs = out if isinstance(out, (tuple, list)) else (out,)
+        sum((o.float() * torch.randn_like(o.float())).mean() for o in outs).backward()
+    launches = _record(run)
+    del m
+    return launches
 
 
 def _sms():
@@ -263,6 +322,104 @@ def _replay_split_f32(a, null, g):
     return {"dtype": "fp32", "kernel": "split_f32", "grid": 0, "items": 0, "worst": worst}, fails
 
 
+def _replay_conv_direct(a, null, g):
+    """CUDA-core convolution, one CTA per 16 x 16 pixels x 16 output channels.  With a bias it is a forward: w [CoutStore, C0 + C1]
+    through the 'wf' pack, the sources split at C0.  Without one it is a data gradient as the executors call it: the operand is dY
+    with C0 = the layer's padded Cout channels, the layer's weight [C0, CoutStore] goes through its 'wd' pack (taps flipped, roles
+    swapped) and CoutStore is the source slice width."""
+    C0, C1, sd, om, N, H, W = a["C0"], a["C1"], a["src_f32"], a["out_mode"], a["N"], a["H"], a["W"]
+    CinP, CoutP, Cs, ks = a["CinP"], a["CoutP"], a["CoutStore"], a["ksize"]
+    Cin, dgrad = C0 + C1, "bias" in null
+    scale = _scales(Cin, g)
+    x = (torch.randn(N, H, W, Cin, device=DEV, generator=g) * scale).to(DTYPE[sd])
+    bias = b64 = None
+    if dgrad:
+        wl = torch.randn(C0, Cs, ks, ks, device=DEV, generator=g) / math.sqrt(C0 * ks * ks)     # the layer's weight [Cout, slice]
+        pk = pack_conv_weights(wl, [Cs])
+        assert C1 == 0 and pk["CoutP"] == CinP and len(pk["wd"][0]) == ks * ks * CinP * CoutP
+        wpk, w64 = pk["wd"][0], wl.double().flip(2, 3).transpose(0, 1)
+    else:
+        w = torch.randn(Cs, Cin, ks, ks, device=DEV, generator=g) / math.sqrt(Cin * ks * ks)
+        pk = pack_conv_weights(w, [C0, C1] if C1 else [C0])
+        assert pk["CinP"] == CinP and pk["CoutP"] == CoutP
+        wpk, w64 = pk["wf"], w.double()
+        b = _bias(scale, w64, g)
+        bias = torch.zeros(CoutP, device=DEV)
+        bias[:Cs] = b
+        b64 = b.double()
+    s0 = x[..., :C0].contiguous()
+    s1 = x[..., C0:].contiguous() if C1 else None
+    out = torch.full((N, Cs, H, W) if om == 1 else (N, H, W, Cs), float("nan"), device=DEV, dtype=OUT_T[om])
+    call("wsl_conv_direct", s0, C0, s1, C1, sd, wpk, bias, out, om, N, H, W, CinP, CoutP, Cs, ks)
+    torch.cuda.synchronize()
+    tiling = CC.Tiling(H, W, 16, 16, 16) if H % 16 == 0 and W % 16 == 0 else None
+    K = ks * ks * Cin
+    rep, _ = _check_conv_output(x, w64, b64, 1, out, om, CC.direct_u(OUT_T[om]), CC.direct_slack(K), tiling, False)
+    items = N * -(-H // 16) * -(-W // 16)
+    row = {"dtype": DTN[sd], "kernel": "conv_direct", "grid": items, "items": items, "NT": 16, "worst": rep["worst"],
+           "out_mode": om, "sources": 2 if C1 else 1, "form": "dgrad" if dgrad else "fwd", "K": K}
+    return row, ([] if rep["bad"] == 0 else [CC.describe(rep)])
+
+
+def _direct_splits(CoutP, Cin, ntiles):
+    """the host dispatch of wsl_wgrad_direct: split count of the pixel tiles"""
+    ob = (CoutP // 16) * -(-Cin // 16)
+    return max(1, min(-(-_sms() * 6 // ob), ntiles))
+
+
+def _replay_wgrad_direct(a, null, g):
+    """CUDA-core weight gradient: CTA (16 co, 16 ci, split) sums its split's 8 x 16 pixel tiles; dw and dbias accumulate atomically"""
+    C0, C1, sd, dd = a["C0"], a["C1"], a["src_f32"], a["dy_f32"]
+    CoutP, N, H, W, Cr, ks = a["CoutP"], a["N"], a["H"], a["W"], a["CoutReal"], a["ksize"]
+    Cin, P = C0 + C1, a["N"] * a["H"] * a["W"]
+    x = (torch.randn(N, H, W, Cin, device=DEV, generator=g) * _scales(Cin, g)).to(DTYPE[sd])
+    # dY per channel: scale 2^-4 .. 2^4 and a mean two standard deviations from zero, so that the signed sum dbias moves by a
+    # split's share when a split is lost (zero-mean dY would leave that share near the noise of the sum)
+    mean = torch.where(torch.rand(Cr, device=DEV, generator=g) < 0.5, -2.0, 2.0)
+    dy = torch.zeros(N, H, W, CoutP, device=DEV, dtype=DTYPE[dd])
+    dy[..., :Cr] = ((torch.randn(N, H, W, Cr, device=DEV, generator=g) + mean) * _scales(Cr, g)).to(DTYPE[dd])
+    s0 = x[..., :C0].contiguous()
+    s1 = x[..., C0:].contiguous() if C1 else None
+    ref = _wgrad_reference(x, dy, Cr, ks, 1)
+    db_ref = dy[..., :Cr].double().sum((0, 1, 2))
+    db_mag = dy[..., :Cr].double().abs().sum((0, 1, 2))
+    ntiles = N * -(-W // 16) * -(-H // 8)
+    row = {"dtype": DTN[dd], "kernel": "wgrad_direct", "grid": _direct_splits(CoutP, Cin, ntiles), "items": ntiles,
+           "src": DTN[sd], "sources": 2 if C1 else 1, "dbias": "dbias" not in null}
+    fails = []
+    margin = CC.chunks_missing_margin(P)              # one 8 x 16 pixel tile left out of P pixels
+    row["margin"] = margin / CC.WGRAD_TOL
+    if margin < 50 * CC.WGRAD_TOL:
+        fails.append(f"one 8 x 16 tile of {P} pixels moves dw by {margin:.1e}, under 50x the {CC.WGRAD_TOL} bound")
+    if row["dbias"]:
+        # dbias is one atomic per (split, channel) from the ci block 0 CTAs: the smallest split's share of the signed sum (the last
+        # split when the tiles divide raggedly) must stand well above the STAT_TOL bound, or a lost or doubled split could pass
+        S = row["grid"]
+        tile = ((torch.arange(N, device=DEV).view(N, 1, 1) * -(-H // 8) + torch.arange(H, device=DEV).view(1, H, 1) // 8) * -(-W // 16)
+                + torch.arange(W, device=DEV).view(1, 1, W) // 16)
+        share = dy[tile % S == S - 1][:, :Cr].double().sum(0).abs()
+        row["db_margin"] = (share / (STAT_TOL * db_mag)).min().item()
+        if row["db_margin"] < DBIAS_MARGIN:
+            fails.append(f"one split's share of dbias is {row['db_margin']:.3g}x the {STAT_TOL} bound, under {DBIAS_MARGIN}x")
+    dw = torch.zeros(Cr, Cin, ks, ks, device=DEV)
+    db = torch.zeros(Cr, device=DEV) if row["dbias"] else None
+    worst = 0.0
+    for k in (1, 2):                                  # the second call adds on top: dw and dbias double
+        call("wsl_wgrad_direct", s0, C0, s1, C1, sd, dy, dd, CoutP, dw, db, N, H, W, Cr, ks)
+        torch.cuda.synchronize()
+        r = CC.check_wgrad(dw, k * ref, 16, 16)
+        worst = max(worst, r["worst"])
+        if r["bad"]:
+            fails.append(f"dw (call {k}) over the bound in (co block, ci block, rel-L2) {r['bad'][:4]}")
+        if db is not None:
+            r = CC.check_sums(db, k * db_ref, k * db_mag)
+            worst = max(worst, r["worst"])
+            if r["bad"]:
+                fails.append(f"dbias (call {k}) over {STAT_TOL} of sum |dY| at channels {r['bad'][:8]}")
+    row["worst"] = worst
+    return row, fails
+
+
 def _wgrad_reference(x, dy, Cr, ks, dil):
     N, H, W, Cin = x.shape
     cn = _chunk(N, H * W * (Cin + dy.shape[3]) * 8 * 2)
@@ -346,7 +503,11 @@ def _replay(key):
     name, scal, null = key
     a = dict(scal)
     g = torch.Generator(device=DEV).manual_seed(zlib.crc32(repr(key).encode()))
-    if name == "wsl_conv_tc_split":
+    if name == "wsl_conv_direct":
+        row, fails = _replay_conv_direct(a, null, g)
+    elif name == "wsl_wgrad_direct":
+        row, fails = _replay_wgrad_direct(a, null, g)
+    elif name == "wsl_conv_tc_split":
         row, fails = _replay_conv_split(a, null, g)
     elif name in CONV:
         row, fails = _replay_conv(name, a, null, g)
@@ -369,15 +530,25 @@ def _replay(key):
 
 
 def _run(config):
+    """-> (rows, failures) of the configuration's launches; a launch another configuration made is not replayed again"""
     if config not in _RESULTS:
-        launches = _harvest(*CONFIGS[config])
+        launches = _KEYS[config] = _harvest(*CONFIGS[config])
         rows, fails = [], []
         for key in launches:
-            row, f = _replay(key)
-            rows.append(row)
-            fails += [f"{row['entry']} {row['shape']} ({row['kernel']}, {row['dtype']}): {m}" for m in f]
+            if key not in _REPLAYS:
+                row, f = _replay(key)
+                _REPLAYS[key] = (row, [f"{row['entry']} {row['shape']} ({row['kernel']}, {row['dtype']}): {m}" for m in f])
+            rows.append(_REPLAYS[key][0])
+            fails += _REPLAYS[key][1]
         _RESULTS[config] = (rows, fails)
     return _RESULTS[config]
+
+
+def _family(r):
+    k = r["kernel"]
+    if k in ("conv_tc2", "conv_row") and "stat_err" not in r:
+        k += " no-stats"
+    return k, r["dtype"]
 
 
 def _print(config, rows):
@@ -388,18 +559,23 @@ def _print(config, rows):
               + (f" RS {r['RS']}" if r.get("RS") else "") + (f" MT {r['MT']} NT {r['NT']}" if r.get("MT") else "")
               + f"  error/bound {r['worst']:.3g}"
               + (f"  BN rows {r['stat_err']:.1e} (mean {r['mean_sigmas']:.1f} sd)" if "stat_err" in r else "")
-              + (f"  bit-identical {r['bit_identical']}" if "bit_identical" in r else ""))
+              + (f"  bit-identical {r['bit_identical']}" if "bit_identical" in r else "")
+              + (f"  out_mode {r['out_mode']} {r['form']} K {r['K']}" if "out_mode" in r else "")
+              + (f"  src {r['src']} dbias {r['dbias']}" if "dbias" in r else "")
+              + (f" (split share {r['db_margin']:.3g}x bound)" if "db_margin" in r else ""))
     fam = {}
     for r in rows:
-        k = (r["kernel"], r["dtype"])
+        k = _family(r)
         fam[k] = max(fam.get(k, 0.0), r["worst"])
     print(f"[{config}] worst error / bound per kernel family: " + ", ".join(f"{k} {d} {v:.3g}" for (k, d), v in sorted(fam.items())))
 
 
 @pytest.mark.parametrize("config", list(CONFIGS))
 def test_every_convolution_launch_of_a_training_step_against_fp64(config):
+    t0 = time.perf_counter()
     rows, fails = _run(config)
     _print(config, rows)
+    print(f"[{config}] {time.perf_counter() - t0:.1f} s (harvest and the replays no earlier configuration made)")
     assert rows, "no convolution launch was recorded"
     assert not fails, "\n".join(fails)
 
@@ -420,6 +596,84 @@ def test_coverage_of_the_multi_tile_paths():
     assert any(r.get("bit_identical") and r["kernel"] == "wgrad_tc3" for r in rows)
     assert {r["kernel"] for r in _run("pnet2d-n12-bf16")[0]} >= {"conv_tc_dil", "wgrad_tc_dil", "conv_tc2", "wgrad_tc"}
     assert {r["kernel"] for r in _run("unet_cct-n12-fp16x3")[0]} >= {"conv_tc_split", "wgrad_tc_split", "split_f32"}
+    # the evaluation forwards: conv_tc2 and the row kernel without BatchNorm rows, at the validation chunk
+    ev = _run("unet-n64-bf16-eval")[0]
+    for k in ("conv_tc2", "conv_row"):
+        assert any(r["kernel"] == k and "stat_err" not in r and r["shape"].startswith("64x") for r in ev), f"no NULL-statistics {k} at N = 64"
+    # the CUDA-core kernels in every form the fp32 mode and the image layer use
+    everything = [r for c in CONFIGS for r in _run(c)[0]]
+    cd = [r for r in everything if r["kernel"] == "conv_direct"]
+    wd = [r for r in everything if r["kernel"] == "wgrad_direct"]
+    print(f"conv_direct: out_mode {sorted({r['out_mode'] for r in cd})}, forms {sorted({r['form'] for r in cd})}, K up to "
+          f"{max(r['K'] for r in cd)}; wgrad_direct: up to {max(r['per_cta'] for r in wd)} tiles per split, "
+          f"{sum(r['ragged'] for r in wd)} of {len(wd)} launches with a ragged split")
+    assert {0, 1, 2, 3} <= {r["out_mode"] for r in cd}, sorted({r["out_mode"] for r in cd})
+    assert any(r["sources"] == 2 for r in cd) and any(r["form"] == "dgrad" for r in cd)
+    assert any(r["dtype"] == "fp32" and r["src"] == "fp32" for r in wd), "no wgrad_direct with dy_f32 = 1"
+    assert {"bf16", "fp16", "fp32"} <= {r["dtype"] for r in wd}, sorted({r["dtype"] for r in wd})
+    assert any(r["dbias"] for r in wd) and any(r["sources"] == 2 for r in wd)
+    print(f"wgrad_direct dbias: smallest split share {min(r['db_margin'] for r in wd if r['dbias']):.3g}x the bound")
+    assert any(r["ragged"] for r in wd), "no wgrad_direct launch splits its tiles raggedly (ntiles % splits != 0)"
+
+
+# ------------------------------------------------------------------------------------------------------------ census
+def _census_inputs(script, recipe, args, B, g):
+    img = torch.rand(B, 1, 256, 256, generator=g).to(DEV)
+    lab = torch.randint(0, 4, (B, 256, 256), generator=g, dtype=torch.uint8)
+    scr = torch.where(torch.rand(B, 256, 256, generator=g) < 0.1, lab, torch.full_like(lab, 4))
+    lab, scr = lab.to(DEV), scr.to(DEV)
+    if recipe.kind == "s2l":
+        return img, scr, torch.softmax(torch.rand(B, 256, 256, 4, generator=g) * 4, -1).to(DEV)
+    if recipe.kind == "semi" and script != "train_partially_fully_supervised.py":
+        return img, lab, torch.rand(B, 1, 256, 256, generator=g).to(DEV)
+    return img, scr if args.sup_type == "scribble" else lab
+
+
+def _census():
+    """{launch key: [where it was made]} over one eager bf16 iteration of every recipe at its own batch, one resident validation pass
+    and one test-step volume"""
+    import numpy as np
+    from wsl4mis_b200 import test_2D, train, val_2D
+    from wsl4mis_b200.networks.net_factory import net_factory
+    seen = {}
+
+    def note(launches, where):
+        for key in launches:
+            seen.setdefault(key, []).append(where)
+    for script, recipe in train.RECIPES.items():
+        args = train.parser_for(script).parse_args([])
+        B = train.rank_batch(script, args.batch_size, 1)
+        torch.manual_seed(0)
+        model = net_factory(net_type=args.model, in_chns=1, class_num=args.num_classes).set_precision("bf16")
+        step = recipe.step(args, model, 1)
+        step.graph_enabled = False
+        inputs = _census_inputs(script, recipe, args, B, torch.Generator().manual_seed(len(script)))
+        note(_record(lambda: step(*inputs)), f"{script} at batch {B}")
+        del model, step, inputs
+    net = UNet(1, 4).to(DEV).set_precision("bf16")
+    rs = np.random.RandomState(5)
+    shapes = [(30, 200, 180), (25, 256, 256), (20, 212, 240)]
+    vs = val_2D.ValidationSet.from_arrays([rs.rand(*s).astype(np.float32) for s in shapes],
+                                          [rs.randint(0, 4, s).astype(np.uint8) for s in shapes])
+    note(_record(lambda: vs.predict(net)), f"validation pass (chunk {vs.chunk})")
+    vol = rs.rand(20, 230, 210).astype(np.float32)
+    note(_record(lambda: test_2D.predict_volume(vol, net)), f"test step (chunk {test_2D.CHUNK})")
+    del net, vs
+    return seen
+
+
+def test_census_every_convolution_launch_of_the_recipes_is_replayed():
+    """the harvest above is complete: every convolution launch the recipes' steps, the validation pass and the test step make is
+    one of the replayed launches"""
+    seen = _census()
+    replayed = set()
+    for c in CONFIGS:
+        _run(c)
+        replayed |= set(_KEYS[c])
+    missing = {k: w for k, w in seen.items() if k not in replayed}
+    print(f"\ncensus: {len(seen)} distinct convolution launches, {len(seen) - len(missing)} replayed")
+    assert not missing, "launches no configuration replays:\n" + "\n".join(
+        f"  {k[0]} {dict(k[1])} NULL {list(k[2])}  <- {', '.join(sorted(set(w)))}" for k, w in sorted(missing.items(), key=repr))
 
 
 def test_conv_tc2_rejects_fp32_nhwc_output():
@@ -431,3 +685,24 @@ def test_conv_tc2_rejects_fp32_nhwc_output():
         call("wsl_conv_tc2", x, 16, None, 0, pk["bf"], None, out, 2, 1, 16, 128, 16, 16, 3, 0, None, None)
     torch.cuda.synchronize()
     assert not out.any()
+
+
+@pytest.mark.parametrize("out_mode", [0, 3, 4])
+def test_conv_direct_rejects_a_partial_16_bit_channel_group(out_mode):
+    """the 16-bit epilogue stores whole 8-channel groups, so CoutStore % 8 != 0 in out_mode 0 / 3 (and any out_mode beyond 3) is an
+    error that leaves the output untouched, not a silently unwritten tail"""
+    x = torch.randn(1, 16, 16, 16, device=DEV).to(torch.bfloat16)
+    w = torch.randn(12, 16, 3, 3, device=DEV) / 12
+    pk = pack_conv_weights(w, [16])
+    out = torch.zeros(1, 16, 16, 12, device=DEV, dtype=torch.float16 if out_mode == 3 else torch.bfloat16)
+    with pytest.raises(RuntimeError, match="CoutStore"):
+        call("wsl_conv_direct", x, 16, None, 0, 0, pk["wf"], None, out, out_mode, 1, 16, 16, 16, 16, 12, 3)
+    torch.cuda.synchronize()
+    assert not out.any()
+    # the same 12 channels stored as fp32 NHWC are written whole
+    out = torch.full((1, 16, 16, 12), float("nan"), device=DEV)
+    call("wsl_conv_direct", x, 16, None, 0, 0, pk["wf"], None, out, 2, 1, 16, 16, 16, 16, 12, 3)
+    torch.cuda.synchronize()
+    ref, S = CC.reference(x.permute(0, 3, 1, 2).double(), w.double(), None)
+    rep = CC.check_output(out.permute(0, 3, 1, 2).double(), ref, S, CC.direct_u(torch.float32), CC.direct_slack(144))
+    assert rep["bad"] == 0, CC.describe(rep)

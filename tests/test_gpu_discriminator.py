@@ -1,13 +1,15 @@
 """FCDiscriminator on the H100 (reference networks/discriminator.py:58-101): the space-to-depth packers bit for bit against the CPU
-oracle, every tensor-core launch of the plan at the DAN script's shapes against fp64 on the same 16-bit operands, both modes against the
-oracle, and one full DAN iteration (train_deep_adversarial_network_2D.py:138-178) in fp32 mode."""
+oracle, every convolution launch of the plan (tensor-core in bf16, CUDA-core in fp32) at the DAN script's shapes against fp64 on the
+same operands, both modes against the oracle, and one full DAN iteration (train_deep_adversarial_network_2D.py:138-178) in fp32
+mode."""
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
 import dan_oracle as D
-from _conv_check import SLACK_16, UNIT_ROUNDOFF, check_output, check_wgrad, describe, reference, wgrad_reference
+from _conv_check import (SLACK_16, UNIT_ROUNDOFF, check_output, check_wgrad, describe, direct_slack, direct_u, reference,
+                         wgrad_reference)
 from _gpu_util import ENC_MASK_KEYS, elem_masks_nchw, rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -70,32 +72,50 @@ def test_packers_and_gathers_bit_exact():
 def test_tensor_core_launches_against_fp64(N):
     """forward, data gradient and weight gradient of every layer on the bf16 tensor-core kernels, with the operands the executor
     produced at the DAN script's batch sizes (phase 1: B = 6, phase 2: 2B = 12)"""
-    m = _model("bf16")
+    _layer_launches_against_fp64(N, "bf16")
+
+
+@pytest.mark.parametrize("N", [6, 12])
+def test_direct_kernel_launches_against_fp64(N):
+    """the same in fp32 mode, on the CUDA-core wsl_conv_direct / wsl_wgrad_direct: the last layer reads 1024 channels (K = 9216
+    sequential FMAs per output, and 2048 weight-gradient CTAs)"""
+    _layer_launches_against_fp64(N, "fp32")
+
+
+def _layer_launches_against_fp64(N, precision):
+    m = _model(precision)
     m.train()
     mp, feat = D.synth_inputs(5, N)
     m.channel_keep = D.chan_keep(6, N)
     ex = m.executor
     logits, rec = ex.forward(mp.to(DEV), feat.to(DEV), True, True, True, m.channel_keep)
     g = torch.Generator(device=DEV).manual_seed(N)
-    u = UNIT_ROUNDOFF[torch.bfloat16]
+    f32 = precision == "fp32"
+    u = direct_u(torch.float32) if f32 else UNIT_ROUNDOFF[torch.bfloat16]
     for i, L in enumerate(ex.layers):
         fwd, dgr, bias = rec["packs"][i]
         T, y = rec["Ts"][i], rec["ys"][i]
-        w3 = fwd.view(9, L.Cout, L.CP).permute(1, 2, 0).reshape(L.Cout, L.CP, 3, 3).double()     # [taps][Cout][Cin] -> torch layout
+        if f32:       # 'wf' pack [taps][CinP][CoutP] -> torch layout
+            w3 = fwd.view(9, L.CP, L.Cout).permute(2, 1, 0).reshape(L.Cout, L.CP, 3, 3).double()
+        else:         # wgmma B operand [taps][Cout][Cin] -> torch layout
+            w3 = fwd.view(9, L.Cout, L.CP).permute(1, 2, 0).reshape(L.Cout, L.CP, 3, 3).double()
         ref, S = reference(_nchw(T), w3, bias.double())
-        rep = check_output(_nchw(y), ref, S, u, SLACK_16)
+        rep = check_output(_nchw(y), ref, S, u, direct_slack(9 * L.CP) if f32 else SLACK_16)
         assert rep["bad"] == 0, f"layer {i} forward (N={N}): {describe(rep)}"
-        dy = (torch.randn(y.shape, generator=g, device=DEV) * 0.1).to(torch.bfloat16)
+        fw = rep["worst"]
+        dy = torch.randn(y.shape, generator=g, device=DEV) * 0.1
+        dy = dy if f32 else dy.to(torch.bfloat16)
         dT = ex._dgrad(L, dy, dgr, N)
         ref, S = reference(_nchw(dy), w3.flip(2, 3).transpose(0, 1), None)
-        rep = check_output(_nchw(dT), ref, S, u, SLACK_16)
+        rep = check_output(_nchw(dT), ref, S, u, direct_slack(9 * L.Cout) if f32 else SLACK_16)
         assert rep["bad"] == 0, f"layer {i} data gradient (N={N}): {describe(rep)}"
         dws, db = ex._wgrad(L, T, dy, N)
         dw_ref = D.gather(wgrad_reference(_nchw(T), _nchw(dy), 3), L.C)
         rw = check_wgrad(torch.cat(dws, 1), dw_ref, 64, L.C)
         assert not rw["bad"], f"layer {i} weight gradient (N={N}): {rw}"
         assert rel_l2(db, _nchw(dy).sum((0, 2, 3))) < 1e-5, f"layer {i} bias gradient"
-        print(f"[disc tc N={N}] layer {i}: wgrad rel-L2 {rw['rel']:.2e}")
+        print(f"[disc {precision} N={N}] layer {i} ({L.CP} -> {L.Cout} at {L.h}x{L.h}): error / bound forward {fw:.3g}, data gradient "
+              f"{rep['worst']:.3g}; wgrad rel-L2 {rw['rel']:.2e}")
 
 
 def _oracle_run(p, mp, feat, training, keep, quant=None, dtype=torch.float64):

@@ -1,6 +1,6 @@
 """Every non-convolution launch of a training step (BatchNorm statistics / finalize / activation / pooling / backward, upsample,
-channel dropout, feature noise, deep-supervision resize, LeakyReLU, layout conversion, weight packing, the first layer's CUDA-core
-convolution), replayed at the step's own shapes in every storage type and checked per element against fp64
+channel dropout, feature noise, deep-supervision resize, LeakyReLU, layout conversion, weight packing, the first layer's conv_first
+and its weight gradient), replayed at the step's own shapes in every storage type and checked per element against fp64
 (tests/_netop_check.py states the bounds and the counter-RNG restatement).
 
 The launches are harvested as tests/test_gpu_conv_at_scale.py harvests the convolutions: one eager forward (+ backward) per
@@ -17,10 +17,9 @@ dw must double), wsl_bn_bwd once more with g0 = NULL (MODE 4), and the synchroni
 whole batch.
 
 Bounds specific to this file (the others are in _netop_check):
-  * conv_first and the single-channel conv_direct (PNet2D's first layer): 9 fp32 FMAs + bias, so |got - ref| <= u_T |ref| + 2^-19 S (10 roundings of at
-    most S = conv(|x|, |w|) + |b|);
-    its BatchNorm rows and wgrad_first / bn_bwd_first / wgrad_direct's dw as the convolution scale test checks them
-    (STAT_TOL, rel-L2 1e-4).
+  * conv_first: 9 fp32 FMAs + bias, so |got - ref| <= u_T |ref| + 2^-19 S (10 roundings of at most S = conv(|x|, |w|) + |b|);
+    its BatchNorm rows and wgrad_first / bn_bwd_first's dw as the convolution scale test checks them (STAT_TOL, rel-L2 1e-4).
+    The CUDA-core wsl_conv_direct / wsl_wgrad_direct, PNet2D's image layer included, are the convolution scale test's.
   * upsample forward: six fp32 roundings of a convex combination (< 2^-21 M, M = the largest of the source neighbourhood) and
     lam = ratio * Y - base formed in fp32 (ratio rounded, the product rounded: off by <= 2^-23 h), which moves the output by
     <= 2^-22 h M per axis: |got - ref| <= u_T |ref| + (2^-21 + 2^-22 (h + w)) M.
@@ -45,7 +44,7 @@ import torch.nn.functional as F
 
 import _conv_check as CC
 import _netop_check as K
-from _gpu_util import LaunchRecorder, pack_conv_weights
+from _gpu_util import LaunchRecorder
 from test_gpu_conv_at_scale import HARVESTED as CONV_HARVESTED
 
 pytestmark = pytest.mark.gpu
@@ -672,63 +671,6 @@ def _replay_conv_first(a, null, g, N_cfg):
     return row, fails
 
 
-def _replay_conv_direct(a, null, g, N_cfg):
-    """the CUDA-core convolution of a single-channel fp32 image (PNet2D's first layer); one CTA per 16 x 16 pixels x 16 channels"""
-    C0, C1, sf, om, N, H, W = a["C0"], a["C1"], a["src_f32"], a["out_mode"], a["N"], a["H"], a["W"]
-    CinP, CoutP, Cs, ks = a["CinP"], a["CoutP"], a["CoutStore"], a["ksize"]
-    odt = {0: 0, 1: 1, 2: 1, 3: 2}[om]
-    row = {"dtype": DTN[odt], "grid": N * -(-H // 16) * -(-W // 16) * (CoutP // 16), "iters": 1, "tail": False, "family": "conv_direct",
-           "worst": 0.0}
-    if not (sf == 1 and C0 == 1 and C1 == 0):
-        return row, ["replayed for the single-channel image layer only"]
-    x = _image(N, H, W, g)
-    w = torch.randn(Cs, 1, ks, ks, device=DEV, generator=g) / ks
-    pk = pack_conv_weights(w, [1])
-    assert pk["CinP"] == CinP and pk["CoutP"] == CoutP
-    bias = b64 = None
-    if "bias" not in null:
-        bias = torch.zeros(CoutP, device=DEV)
-        bias[:Cs] = torch.randn(Cs, device=DEV, generator=g)
-        b64 = bias[:Cs].double()
-    shape = (N, Cs, H, W) if om == 1 else (N, H, W, Cs)
-    out = torch.full(shape, math.nan, device=DEV, dtype=K.TORCH_T[odt])
-    call("wsl_conv_direct", x, 1, None, 0, 1, pk["wf"], bias, out, om, N, H, W, CinP, CoutP, Cs, ks)
-    torch.cuda.synchronize()
-    ref, S = CC.reference(x[:, None].double(), w.double(), b64)
-    got = out.double() if om == 1 else out.permute(0, 3, 1, 2).double()
-    rep = CC.check_output(got, ref, S, K.U[odt], 2.0 ** -19, CC.Tiling(H, W, 16, 16, 16))
-    row["worst"] = rep["worst"]
-    return row, ([] if rep["bad"] == 0 else [CC.describe(rep)])
-
-
-def _replay_wgrad_direct(a, null, g, N_cfg):
-    """weight (+ bias) gradient of the same single-channel image convolution; dw and dbias accumulate"""
-    C0, C1, sf, N, H, W = a["C0"], a["C1"], a["src_f32"], a["N"], a["H"], a["W"]
-    CoutP, Cr, ks, ddt = a["CoutP"], a["CoutReal"], a["ksize"], a["dy_f32"]
-    row = {"dtype": DTN[ddt], "grid": 0, "iters": 0, "tail": False, "family": "wgrad_direct", "worst": 0.0}
-    if not (sf == 1 and C0 == 1 and C1 == 0):
-        return row, ["replayed for the single-channel image layer only"]
-    fails = []
-    x = _image(N, H, W, g)
-    dy = torch.zeros(N, H, W, CoutP, device=DEV, dtype=K.TORCH_T[ddt])
-    dy[..., :Cr] = _grad((N, H, W, Cr), Cr, ddt, g)
-    ref = CC.wgrad_reference(x[:, None].double(), dy[..., :Cr].permute(0, 3, 1, 2).double(), ks)
-    dbias_ref = dy[..., :Cr].double().sum((0, 1, 2))
-    dbias_mag = dy[..., :Cr].double().abs().sum((0, 1, 2))
-    dw = torch.zeros(Cr, 1, ks, ks, device=DEV)
-    db = None if "dbias" in null else torch.zeros(Cr, device=DEV)
-    for k in (1, 2):                                          # the second call adds on top
-        call("wsl_wgrad_direct", x, 1, None, 0, 1, dy, ddt, CoutP, dw, db, N, H, W, Cr, ks)
-        torch.cuda.synchronize()
-        r = CC.check_wgrad(dw, k * ref, 16, 1)
-        row["worst"] = max(row["worst"], r["worst"])
-        if r["bad"]:
-            fails.append(f"dw (call {k}) over the bound in (co block, -, rel-L2) {r['bad'][:4]}")
-        if db is not None:
-            _merge([K.sums(db, k * dbias_ref, k * dbias_mag, what=f"dbias (call {k})")], fails, row)
-    return row, fails
-
-
 def _replay_wgrad_first(a, null, g, N_cfg):
     N, H, W, dt = a["N"], a["H"], a["W"], a["dtype"]
     b = max(1, min(-(-(N * H * W) // 4096), _sms()))
@@ -1047,8 +989,6 @@ REPLAY = {
     "wsl_bn_bwd_coef": _replay_bn_bwd_coef,
     "wsl_bn_bwd_first": _replay_bn_bwd_first,
     "wsl_conv_first": _replay_conv_first,
-    "wsl_conv_direct": _replay_conv_direct,
-    "wsl_wgrad_direct": _replay_wgrad_direct,
     "wsl_wgrad_first": _replay_wgrad_first,
     "wsl_upsample2x_fwd": lambda *r: _replay_upsample("wsl_upsample2x_fwd", *r),
     "wsl_upsample2x_bwd": lambda *r: _replay_upsample("wsl_upsample2x_bwd", *r),

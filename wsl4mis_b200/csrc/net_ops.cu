@@ -1552,6 +1552,10 @@ WSL_API int wsl_conv_direct(const void* src0, int C0, const void* src1, int C1, 
   WSL_REQUIRE(ksize == 3 || ksize == 1, "wsl_conv_direct: ksize must be 1 or 3");
   WSL_REQUIRE(CinP % 16 == 0 && CoutP % 16 == 0, "wsl_conv_direct: padded channel counts must be multiples of 16");
   WSL_REQUIRE((src_f32 == 1 && C1 == 0) || (C0 % 8 == 0 && C1 % 8 == 0), "wsl_conv_direct: multi-channel sources need C %% 8 == 0");
+  // the 16-bit epilogue stores whole 8-channel groups: a partial last group would be left unwritten
+  WSL_REQUIRE(out_mode == 1 || out_mode == 2 || ((out_mode == 0 || out_mode == 3) && CoutStore % 8 == 0),
+              "wsl_conv_direct: out_mode %d with CoutStore %d (16-bit NHWC outputs need CoutStore %% 8 == 0; out_mode is 0 .. 3)",
+              out_mode, CoutStore);
   const int tx = (W + 15) / 16, ty = (H + 15) / 16;
   dim3 grid(N * tx * ty, CoutP / 16);
   if (ksize == 3)
