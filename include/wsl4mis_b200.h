@@ -279,10 +279,8 @@ int wsl_bn_finalize(const float* partials, int nrows, long long P, int C, const 
  * Bias gradients are NOT produced here (see wsl_channel_sum). */
 int wsl_wgrad_tc(const void* src0, int C0, const void* src1, int C1, const void* dy, int CoutP, float* dw, int N, int H,
                  int W, int CoutReal, int ksize, int dtype, float* partial_ws, long long partial_floats, cudaStream_t stream);
-/* v2 of the 3x3 weight gradient: one halo load of X per 16x8 pixel chunk, nine row-shifted descriptor views. */
-int wsl_wgrad_tc2(const void* src0, int C0, const void* src1, int C1, const void* dy, int CoutP, float* dw, int N, int H,
-                  int W, int CoutReal, int ksize, int dtype, cudaStream_t stream);
-/* v3: filter columns ride in the MMA's M dimension (A = X halo with one-pixel group stride, B = dY, N = Cout tile). */
+/* the 3x3 weight gradient with the filter columns in the MMA's M dimension (A = X halo with one-pixel group stride, B = dY,
+ * N = Cout tile); needs W % 8 == 0, H % 16 == 0 and CoutP 16, 32, 64 or a multiple of 128. */
 int wsl_wgrad_tc3(const void* src0, int C0, const void* src1, int C1, const void* dy, int CoutP, float* dw, int N, int H,
                   int W, int CoutReal, int ksize, int dtype, float* partial_ws, long long partial_floats, cudaStream_t stream);
 /* partial_ws (optional, partial_floats floats): split-K partial tiles go there and a fixed-order finalize adds them into dw -> the
@@ -351,14 +349,6 @@ int wsl_bn_act_fwd_ps(const void* y, int dtype, const float* ss, int N, int H, i
 int wsl_bn_act_fwd(const void* y, int dtype, const float* ss, int N, int H, int W, int C, float slope, float drop_p,
                    const uint8_t* mask, unsigned long long seed, const unsigned long long* seed_ptr, void* act,
                    void* pooled, uint8_t* pool_idx, cudaStream_t stream);
-
-/* the same with wsl_bn_finalize folded in (C <= 32): every block derives {scale, shift} from the convolution epilogue's partial rows,
- * block 0 publishes save / ss / running statistics; one launch less on the forward critical path of the full-resolution layers. */
-int wsl_bn_finalize_act_fwd(const void* y, int dtype, const float* partials, int nrows, const float* gamma, const float* beta,
-                            float* running_mean, float* running_var, long long* num_batches_tracked, float momentum, float eps,
-                            float* save, float* ss, int N, int H, int W, int C, float slope, float drop_p, const uint8_t* mask,
-                            unsigned long long seed, const unsigned long long* seed_ptr, void* act, void* pooled,
-                            uint8_t* pool_idx, cudaStream_t stream);
 
 /* backward of the same chain: dA = g0 + cs1*g1 + maxpool-routed gpool (each optional) -> dY, dgamma, dbeta (added to the
  * existing values when accumulate != 0: a second backward through shared weights, e.g. the mean-teacher student). */

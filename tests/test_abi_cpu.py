@@ -39,7 +39,7 @@ def test_no_undeclared_exports(lib_path):
 
 def test_abi_version_and_workspace(lib_path):
     dll = _lib.LIB.load()
-    assert dll.wsl_abi_version() == 1
+    assert dll.wsl_abi_version() == 2
     assert dll.wsl_workspace_floats() >= 1 << 16
 
 

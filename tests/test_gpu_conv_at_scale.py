@@ -45,7 +45,7 @@ if torch.cuda.is_available():
     from wsl4mis_b200.networks.unet import UNet, UNet_CCT
 
 CONV = ("wsl_conv_tc", "wsl_conv_tc_dil", "wsl_conv_tc2", "wsl_conv_tc_split")
-WGRAD = ("wsl_wgrad_tc", "wsl_wgrad_tc2", "wsl_wgrad_tc3", "wsl_wgrad_tc_dil", "wsl_wgrad_tc_split")
+WGRAD = ("wsl_wgrad_tc", "wsl_wgrad_tc3", "wsl_wgrad_tc_dil", "wsl_wgrad_tc_split")
 DIRECT = ("wsl_conv_direct", "wsl_wgrad_direct")
 HARVESTED = CONV + WGRAD + DIRECT + ("wsl_split_f32",)
 T16 = {0: torch.bfloat16, 2: torch.float16}
@@ -142,7 +142,7 @@ def _n_tile(CoutP):
 
 
 def _conv_tc2_plan(C0, C1, N, H, W, CoutP, ks):
-    """the host dispatch of wsl_conv_tc2 (default settings): row kernel or halo kernel, its tile and N tile"""
+    """the host dispatch of wsl_conv_tc2: row kernel or halo kernel, its tile and N tile"""
     if ks == 3 and CoutP in (16, 32) and W % 128 == 0 and H % 16 == 0 and C0 + C1 <= 64:
         RS = 32 if H % 32 == 0 and N * (W // 128) * (H // 32) >= 4 * _sms() else 16
         return {"kernel": "conv_row", "th": RS, "tw": 128, "nt": CoutP, "order": "xy", "items": N * (W // 128) * (H // RS), "RS": RS}

@@ -169,14 +169,14 @@ WGRAD_TC_CASES += [(2, 32, 32, 16, 0, 16, 3), (1, 64, 32, 32, 32, 32, 3), (2, 32
 
 
 @pytest.mark.parametrize("case", WGRAD_TC_CASES)
-@pytest.mark.parametrize("ver", ["wsl_wgrad_tc", "wsl_wgrad_tc2", "wsl_wgrad_tc3", "wsl_wgrad_tc3-fp16"])
+@pytest.mark.parametrize("ver", ["wsl_wgrad_tc", "wsl_wgrad_tc3", "wsl_wgrad_tc3-fp16"])
 def test_wgrad_tc(case, ver):
     """wgmma weight gradient vs fp64 autograd on the same 16-bit inputs; fp32 accumulation -> 1e-4 relative."""
     N, H, W, C0, C1, Cout, ks = case
     dt = 2 if ver.endswith("-fp16") else 0
     ver = ver.split("-")[0]
     if ver != "wsl_wgrad_tc" and (ks != 3 or H % 16 or W % 8):
-        pytest.skip("v2: 3x3, 8x16 chunks")
+        pytest.skip("v3: 3x3, 8x16 chunks")
     if ver == "wsl_wgrad_tc" and (H % 8 or W % 16):
         pytest.skip("v1: 16x8 chunks")
     g = torch.Generator().manual_seed(17)

@@ -56,7 +56,7 @@ if torch.cuda.is_available():
     from wsl4mis_b200.networks.pnet import PNet2D
     from wsl4mis_b200.networks.unet import UNet, UNet_CCT, UNet_CCT_3H, UNet_DS
 
-# id -> (model, N, precision, mode); mode: train | sync | folded | per_sample | eval | ds
+# id -> (model, N, precision, mode); mode: train | sync | per_sample | eval | ds
 CONFIGS = {
     "unet_cct-n12-bf16": ("unet_cct", 12, "bf16", "train"),
     "unet_cct-n64-bf16": ("unet_cct", 64, "bf16", "train"),
@@ -64,7 +64,6 @@ CONFIGS = {
     "unet_cct-n12-fp16x3": ("unet_cct", 12, "fp16x3", "train"),
     "unet_cct-n12-bf16-sync": ("unet_cct", 12, "bf16", "sync"),
     "unet_cct-n12-fp16x3-sync": ("unet_cct", 12, "fp16x3", "sync"),
-    "unet_cct-n12-bf16-folded": ("unet_cct", 12, "bf16", "folded"),
     "unet-n64-bf16-per-sample": ("unet", 64, "bf16", "per_sample"),
     "unet-n12-bf16-eval": ("unet", 12, "bf16", "eval"),
     "unet_ds-n12-bf16": ("unet_ds", 12, "bf16", "train"),
@@ -102,8 +101,6 @@ def _harvest(config):
     m = _model(kind).to(DEV).set_precision(precision)
     if mode == "sync":
         m.executor.sync_bn = (1, None)          # one rank: ddp.allreduce_flat is a no-op, the synchronised kernels still run
-    if mode == "folded":
-        m.executor.fold_finalize = True
     x = torch.rand(N, 1, 256, 256, device=DEV)
     rec, saved = LaunchRecorder(_keep), _lib.PROFILE
     _lib.PROFILE = rec
@@ -399,7 +396,7 @@ def _replay_bn_act(name, a, null, g, N_cfg):
     grid = grid_for((items + 1) // 2)
     rows = 256 // cg
     it, tail = _walk(P // 4 if pooled else P, grid * rows, not pooled)
-    fam = {"wsl_bn_act_fwd": "bn_act_fwd", "wsl_bn_act_fwd_ps": "bn_act_fwd_ps", "wsl_bn_finalize_act_fwd": "bn_finalize_act_fwd"}[name]
+    fam = {"wsl_bn_act_fwd": "bn_act_fwd", "wsl_bn_act_fwd_ps": "bn_act_fwd_ps"}[name]
     row = {"dtype": DTN[dt], "grid": grid, "iters": it, "tail": tail, "family": fam + ("+pool" if pooled else ""), "worst": 0.0,
            "drop_p": p}
     fails = []
@@ -415,19 +412,6 @@ def _replay_bn_act(name, a, null, g, N_cfg):
         call(name, y, dt, ss, N, H, W, C, slope, p, mask, a["seed"], sp, act, pl, idx)
         sc = ss[:, :C].repeat_interleave(H * W, 0)
         sh = ss[:, C:].repeat_interleave(H * W, 0)
-    elif name == "wsl_bn_finalize_act_fwd":
-        nrows, mom, eps = a["nrows"], a["momentum"], a["eps"]
-        parts = _rows_of(y, nrows)
-        run = "running_mean" not in null
-        rm0, rv0 = torch.randn(C, device=DEV, generator=g), 0.5 + torch.rand(C, device=DEV, generator=g)
-        nbt0 = torch.tensor([5], dtype=torch.int64, device=DEV)
-        rm, rv, nbt = rm0.clone(), rv0.clone(), nbt0.clone()
-        save, ss = torch.full((2 * C,), math.nan, device=DEV), torch.full((2 * C,), math.nan, device=DEV)
-        call(name, y, dt, parts, nrows, gamma, beta, rm if run else None, rv if run else None, nbt if run else None, mom, eps, save, ss,
-             N, H, W, C, slope, p, mask, a["seed"], sp, act, pl, idx)
-        torch.cuda.synchronize()
-        _finish_stats(row, fails, P, C, y, save, ss, gamma, beta, run, rm, rv, rm0, rv0, nbt, nbt0, mom, eps)
-        sc, sh = ss[:C], ss[C:]
     else:
         save, ss = _save_ss(y, gamma, beta)
         call(name, y, dt, ss, N, H, W, C, slope, p, mask, a["seed"], sp, act, pl, idx)
@@ -983,7 +967,6 @@ REPLAY = {
     "wsl_bn_eval_prepare": _replay_bn_eval_prepare,
     "wsl_bn_act_fwd": lambda *r: _replay_bn_act("wsl_bn_act_fwd", *r),
     "wsl_bn_act_fwd_ps": lambda *r: _replay_bn_act("wsl_bn_act_fwd_ps", *r),
-    "wsl_bn_finalize_act_fwd": lambda *r: _replay_bn_act("wsl_bn_finalize_act_fwd", *r),
     "wsl_bn_bwd": _replay_bn_bwd,
     "wsl_bn_bwd_phase": _replay_bn_bwd_phase,
     "wsl_bn_bwd_coef": _replay_bn_bwd_coef,
@@ -1117,7 +1100,7 @@ def test_coverage_of_the_step_shapes():
               f"{sum(1 for r in rs if r.get('iters', 0) >= 2 and r.get('tail'))} of {len(rs)} launches with >= 2 and a tail")
     # two-pixel unrolled loops must end on their single-pixel tail somewhere; the plain grid-stride loops must walk >= 2 iterations
     # (bn_grid sizes uncapped BatchNorm grids to exactly 24 pixels per thread, so only the capped N = 64 launches reach the tail)
-    for f in ("bn_act_fwd", "bn_act_fwd_ps", "bn_finalize_act_fwd", "bn_bwd", "bn_bwd_first"):
+    for f in ("bn_act_fwd", "bn_act_fwd_ps", "bn_bwd", "bn_bwd_first"):
         assert any(r.get("iters", 0) >= 2 and r.get("tail") for r in fams.get(f, [])), f"no {f} launch walks >= 2 iterations into its tail"
     for f in ("bn_stats", "bn_stats_ps", "bn_bwd_phase", "upsample_fwd", "upsample_bwd", "chan_scale", "lrelu_fwd", "lrelu_bwd",
               "feat_noise_fwd", "feat_noise_bwd", "channel_sum", "conv_first", "wgrad_first", "nearest_fwd", "nearest_bwd",
@@ -1134,6 +1117,6 @@ def test_coverage_of_the_step_shapes():
             "wsl_chan_mask_gen", "wsl_bn_bwd_first", "wsl_bn_bwd_phase", "wsl_bn_bwd_coef", "wsl_bn_finalize", "wsl_bn_stats_ps",
             "wsl_bn_act_fwd_ps", "wsl_conv_first", "wsl_wgrad_first", "wsl_nearest_resize_fwd", "wsl_nearest_resize_bwd",
             "wsl_lrelu_fwd", "wsl_lrelu_bwd", "wsl_uniform_fill", "wsl_feat_noise_fwd", "wsl_feat_noise_bwd",
-            "wsl_pack_conv_weights_batched", "wsl_bn_eval_prepare", "wsl_bn_finalize_act_fwd", "wsl_nchw_f32_to_nhwc", "wsl_channel_sum"}
+            "wsl_pack_conv_weights_batched", "wsl_bn_eval_prepare", "wsl_nchw_f32_to_nhwc", "wsl_channel_sum"}
     assert reached >= want, sorted(want - reached)
     assert any(r["entry"] == "wsl_bn_stats" and "raw_sums" not in r["null"] for r in rows)

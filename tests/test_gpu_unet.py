@@ -304,7 +304,7 @@ def test_wide_rows_take_the_row_kernel_and_match_the_oracle():
             continue
         worst[k] = cosine(named[k].grad.detach().cpu(), ref)
     # convolution weights: tight; BatchNorm affine gradients are cancelling sums over a 2-image batch and sit at 0.90-0.93 on
-    # this input with either convolution kernel (WSL4MIS_CONV_ROW=0 gives the same numbers), so they get the looser bound
+    # this input, so they get the looser bound
     bad = {k: round(v, 4) for k, v in worst.items() if v <= (GRAD_COS_Q if named[k].dim() == 4 else 0.85)}
     print("worst cosines:", sorted(worst.items(), key=lambda kv: kv[1])[:6])
     assert not bad, bad

@@ -22,5 +22,5 @@ int wsl_check_launch(const char* what) {
 }
 
 WSL_API const char* wsl_last_error(void) { return g_err; }
-WSL_API int wsl_abi_version(void) { return 1; }
+WSL_API int wsl_abi_version(void) { return 2; }
 WSL_API int wsl_workspace_floats(void) { return WSL_WS_FLOATS; }

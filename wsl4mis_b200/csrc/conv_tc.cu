@@ -837,142 +837,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const __grid_c
 }
 
 // ================================================================================================
-// wgrad v2 (3x3 only): one halo load of X per 8x16 pixel chunk; the nine tap operands are row-shifted MN-major
-// descriptor views of that halo (same absolute-address swizzle argument as conv_tc2).  CTA = (Cout tile of 128) x
-// (Cin block of CWB <= 32) x all nine taps -> nine accumulators of CWB columns (9*CWB/2 registers per consumer thread).
-// L2->SM traffic per chunk: dY tile + 1.4x X block instead of dY + 9 X boxes.
-// ================================================================================================
-template <int CWA, int NA, int CWB, int STAGES>
-struct Wgrad2Smem {
-  static constexpr int A_BOX = TILE_M * CWA * 2;
-  static constexpr int ROWB = CWB * 2;
-  static constexpr int B_HALO = ((10 * 18 * ROWB + 1023) / 1024) * 1024;
-  static constexpr int STAGE_BYTES = ((NA * A_BOX + B_HALO + 1023) / 1024) * 1024;
-  static constexpr int SLACK = (64 / CWA) * A_BOX;
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + SLACK + 1024 + 256;
-};
-
-template <int CWA, int NA, int CWB, int STAGES, int DT>
-__global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc2_kernel(const __grid_constant__ CUtensorMap map_dy,
-                                                                   const __grid_constant__ CUtensorMap map_x0,
-                                                                   const __grid_constant__ CUtensorMap map_x1, const WgradTcParams p) {
-  using S = Wgrad2Smem<CWA, NA, CWB, STAGES>;
-  constexpr int SWA = CWA * 2, SWB = CWB * 2;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES + S::SLACK);
-  uint64_t* empty_bar = full_bar + STAGES;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_tiles = p.n_tiles0 + p.n_tiles1;
-  const int nt = blockIdx.y % n_tiles;
-  const int mt = blockIdx.y / n_tiles;
-  const int m0 = mt * 128;
-  const bool src1 = nt >= p.n_tiles0;
-  const int cb0 = (src1 ? nt - p.n_tiles0 : nt) * CWB;
-  const int ci_global = (src1 ? p.C0 : 0) + cb0;
-  const int my_chunks = (p.nchunks - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_WARPS); }
-    fence_barrier_init();
-    prefetch_tmap(&map_dy);
-    prefetch_tmap(src1 ? &map_x1 : &map_x0);
-  }
-  __syncthreads();
-
-  if (warp >= PRODUCER_WARP) {
-    producer_regs();
-    if (warp != PRODUCER_WARP) return;
-    if (lane == 0) {
-      const CUtensorMap* mx = src1 ? &map_x1 : &map_x0;
-      for (int it = 0; it < my_chunks; ++it) {
-        const int chunk = blockIdx.x + it * gridDim.x;
-        const int n = chunk / (p.tiles_x * p.tiles_y);
-        const int tr = chunk - n * p.tiles_x * p.tiles_y;
-        const int y0 = (tr / p.tiles_x) * 16, x0 = (tr % p.tiles_x) * 8;
-        const int s = it % STAGES;
-        mbar_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
-        uint8_t* a_dst = smem + s * S::STAGE_BYTES;
-        uint8_t* b_dst = a_dst + NA * S::A_BOX;
-        mbar_expect_tx(&full_bar[s], NA * S::A_BOX + 10 * 18 * S::ROWB);
-#pragma unroll
-        for (int i = 0; i < NA; ++i) tma_load_4d(&map_dy, &full_bar[s], a_dst + i * S::A_BOX, m0 + i * CWA, x0, y0, n);
-        tma_load_4d(mx, &full_bar[s], b_dst, cb0, x0 - 1, y0 - 1, n);
-      }
-    }
-    return;
-  }
-  consumer_regs();
-  const int h = threadIdx.x >> 7, t = threadIdx.x & 127;
-  const bool active = m0 + 64 * h < p.CoutP;
-  float acc[9][CWB / 2];
-#pragma unroll
-  for (int tap = 0; tap < 9; ++tap)
-#pragma unroll
-    for (int e = 0; e < CWB / 2; ++e) acc[tap][e] = 0.f;
-  for (int it = 0; it < my_chunks; ++it) {
-    const int s = it % STAGES;
-    mbar_wait(&full_bar[s], (it / STAGES) & 1);
-    if (active) {
-      const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES) + (uint32_t)((64 * h / CWA) * S::A_BOX);
-      const uint32_t b_addr = smem_u32(smem + s * S::STAGE_BYTES + NA * S::A_BOX);
-      wgmma_fence();
-#pragma unroll
-      for (int tap = 0; tap < 9; ++tap) {
-        const int dy = tap / 3, dx = tap % 3;
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          // k-step = 16 pixels = image rows 2k, 2k+1 of the chunk: A advances 16 rows, B advances 2 halo rows
-          Wgmma<CWB>::template mma<1, 1, DT>(acc[tap], gmma_desc<SWA>(a_addr + (uint32_t)(k * 16 * SWA), S::A_BOX, 8 * SWA),
-                                             gmma_desc<SWB>(b_addr + (uint32_t)((dy * 10 + dx) * S::ROWB + k * 2 * 10 * S::ROWB), S::B_HALO, 10 * S::ROWB),
-                                             (it > 0 || k > 0) ? 1u : 0u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-    }
-    release_stage(&empty_bar[s]);
-  }
-  if (my_chunks == 0 || !active) return;
-  const int CinTot = p.C0 + p.C1;
-#pragma unroll
-  for (int tap = 0; tap < 9; ++tap) {
-    wgmma_fence_regs(acc[tap]);
-#pragma unroll
-    for (int ii = 0; ii < 2; ++ii) {
-      const int row = m0 + 64 * h + frag_row(t) + 8 * ii;
-      if (row >= p.CoutReal) continue;
-#pragma unroll
-      for (int e = 0; e < CWB / 4; ++e) {
-        const int c = 8 * (e >> 1) + frag_col(t) + (e & 1);
-        atomicAdd(p.dw + ((size_t)row * CinTot + ci_global + c) * 9 + tap, acc[tap][4 * (e >> 1) + 2 * ii + (e & 1)]);
-      }
-    }
-  }
-}
-
-template <int CWA, int NA, int CWB, int DT>
-int launch_wgrad2(const CUtensorMap& mdy, const CUtensorMap& mx0, const CUtensorMap& mx1, const WgradTcParams& p, int m_tiles,
-                  cudaStream_t stream) {
-  constexpr int per_stage = NA * TILE_M * CWA * 2 + 12 * 1024;
-  constexpr int STAGES = per_stage >= 40 * 1024 ? 3 : 4;
-  using S = Wgrad2Smem<CWA, NA, CWB, STAGES>;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc2_kernel<CWA, NA, CWB, STAGES, DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
-    if (e != cudaSuccess) { wsl_set_error("wgrad_tc2: cudaFuncSetAttribute(%d bytes): %s", S::TOTAL, cudaGetErrorString(e)); return -5; }
-    attr = true;
-  }
-  const int gy = m_tiles * (p.n_tiles0 + p.n_tiles1);
-  int splits = (wsl_num_sms() + gy - 1) / gy;
-  if (splits > p.nchunks) splits = p.nchunks;
-  if (splits < 1) splits = 1;
-  dim3 grid(splits, gy);
-  wgrad_tc2_kernel<CWA, NA, CWB, STAGES, DT><<<grid, NUM_THREADS, S::TOTAL, stream>>>(mdy, mx0, mx1, p);
-  return wsl_check_launch("wgrad_tc2");
-}
-
-// ================================================================================================
 // wgrad v3 (3x3): taps in the M dimension, filter rows in the N dimension.
 //
 //   A := X rows (MN-major).  An M = 64 operand is 64/CWB channel groups spaced LBO apart; with LBO = ONE PIXEL
@@ -1625,8 +1489,7 @@ template <int NT, int KBW, int KB, int DT, int OM>
 int launch_conv_row(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& o, const ConvV2Params& p,
                     int RS, cudaStream_t stream) {
   // Row buffers in flight: ~80 KB per SM cover the HBM latency.
-  static const int st_env = [] { const char* e = getenv("WSL4MIS_ROW_STAGES"); return e ? atoi(e) : 0; }();
-  const int STAGES = st_env ? st_env : (KB == 1 ? 12 : KB == 2 ? 8 : 6);
+  const int STAGES = KB == 1 ? 12 : KB == 2 ? 8 : 6;
   const int w_bytes = ((KB * 9 * NT * KBW * 2 + 1023) / 1024) * 1024;
   const int smem = w_bytes + row_out_bytes(NT) + STAGES * KB * row_abytes(KBW) + 1024 + 256;
   if (smem > 220 * 1024) { wsl_set_error("conv_row: %d bytes of shared memory needed", smem); return -6; }
@@ -1876,14 +1739,12 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
   // 16-bit outputs leave through TMA stores, whose global row pitch must be a multiple of 16 bytes
   WSL_REQUIRE(out_mode != 0 || CoutStore % 8 == 0, "wsl_conv_tc2: 16-bit outputs need CoutStore %% 8 == 0 (got %d)", CoutStore);
   {   // narrow outputs at >= 128-pixel rows: the row kernel (filter rows in N) is 1.8-2.3x faster per pixel
-    static const bool row_on = [] { const char* e = getenv("WSL4MIS_CONV_ROW"); return !(e && e[0] == '0'); }();
-    static const bool wide_on = [] { const char* e = getenv("WSL4MIS_ROW_KBW32"); return !(e && e[0] == '0'); }();
     // channel block per TMA box / swizzle span: 32 channels (64 B) when every source allows it and the output is 32 wide
-    const int kbw = (wide_on && CoutP == 32 && C0 % 32 == 0 && C1 % 32 == 0) ? 32 : 16;
+    const int kbw = (CoutP == 32 && C0 % 32 == 0 && C1 % 32 == 0) ? 32 : 16;
     const int KB = (C0 + C1) / kbw;
     // row segments of 32 output rows (6 % halo re-reads) unless that leaves fewer than ~4 work items per SM
     const int RS = (H % 32 == 0 && (long long)N * (W / ROW_PX) * (H / 32) >= 4 * wsl_num_sms()) ? 32 : 16;
-    if (row_on && ksize == 3 && (CoutP == 16 || CoutP == 32) && W % ROW_PX == 0 && H % 16 == 0 && (C0 + C1) <= 64) {
+    if (ksize == 3 && (CoutP == 16 || CoutP == 32) && W % ROW_PX == 0 && H % 16 == 0 && (C0 + C1) <= 64) {
       CUtensorMap a0, a1, b;
       {
         long long d[4] = {C0, W, H, N};
@@ -2002,53 +1863,7 @@ WSL_API int wsl_conv_tc2(const void* src0, int C0, const void* src1, int C1, con
 #undef WSL_C2
 }
 
-// 3x3 weight gradient, v2 (halo views).  Same contract as wsl_wgrad_tc; needs W % 8 == 0 and H % 16 == 0.
-WSL_API int wsl_wgrad_tc2(const void* src0, int C0, const void* src1, int C1, const void* dy, int CoutP, float* dw, int N, int H,
-                          int W, int CoutReal, int ksize, int dtype, cudaStream_t stream) {
-  WSL_REQUIRE(ksize == 3, "wsl_wgrad_tc2: 3x3 only");
-  WSL_REQUIRE(dtype == 0 || dtype == 2, "wsl_wgrad_tc2: dtype must be 0 (bf16) or 2 (fp16)");
-  WSL_REQUIRE(C0 % 16 == 0 && C1 % 16 == 0 && C0 > 0, "wsl_wgrad_tc2: source channels must be multiples of 16 (got %d,%d)", C0, C1);
-  WSL_REQUIRE(CoutP % 16 == 0 && (CoutP < 128 || CoutP % 128 == 0), "wsl_wgrad_tc2: unsupported CoutP %d", CoutP);
-  WSL_REQUIRE(W % 8 == 0 && H % 16 == 0, "wsl_wgrad_tc2: H,W must be multiples of the 16x8 pixel chunk (got %dx%d)", H, W);
-  const int cwa = CoutP >= 64 ? 64 : CoutP;
-  const int cwb = 16;          // nine accumulators of CWB/2 registers per consumer thread: 16-channel blocks keep them in registers
-  const int na = CoutP >= 128 ? 2 : 1;
-  const int m_tiles = CoutP >= 128 ? CoutP / 128 : 1;
-  CUtensorMap mdy, mx0, mx1;
-  {
-    long long d[4] = {CoutP, W, H, N};
-    int bx[4] = {cwa, 8, 16, 1};
-    int rc = get_map(dy, 4, d, bx, cwa, &mdy, dtype);
-    if (rc) return rc;
-  }
-  {
-    long long d[4] = {C0, W, H, N};
-    int bx[4] = {cwb, 10, 18, 1};
-    int rc = get_map(src0, 4, d, bx, cwb, &mx0, dtype);
-    if (rc) return rc;
-  }
-  if (C1 > 0) {
-    long long d[4] = {C1, W, H, N};
-    int bx[4] = {cwb, 10, 18, 1};
-    int rc = get_map(src1, 4, d, bx, cwb, &mx1, dtype);
-    if (rc) return rc;
-  } else {
-    mx1 = mx0;
-  }
-  WgradTcParams p;
-  p.N = N; p.H = H; p.W = W; p.C0 = C0; p.C1 = C1; p.CoutP = CoutP; p.CoutReal = CoutReal; p.taps = 9; p.ks = 3;
-  p.tiles_x = W / 8; p.tiles_y = H / 16; p.nchunks = N * p.tiles_x * p.tiles_y;
-  p.n_tiles0 = C0 / cwb; p.n_tiles1 = C1 / cwb; p.tap_groups = 1; p.dt = dtype; p.scale_a = nullptr; p.scale_b = nullptr; p.dw = dw; p.partials = nullptr; p.dil = 1;
-  return with_dt(dtype, [&](auto dt) {
-    constexpr int DT = decltype(dt)::value;
-    if (cwa == 64 && na == 2) return launch_wgrad2<64, 2, 16, DT>(mdy, mx0, mx1, p, m_tiles, stream);
-    if (cwa == 64) return launch_wgrad2<64, 1, 16, DT>(mdy, mx0, mx1, p, m_tiles, stream);
-    if (cwa == 32) return launch_wgrad2<32, 1, 16, DT>(mdy, mx0, mx1, p, m_tiles, stream);
-    return launch_wgrad2<16, 1, 16, DT>(mdy, mx0, mx1, p, m_tiles, stream);
-  });
-}
-
-// 3x3 weight gradient, v3 (filter columns in the MMA's M dimension).  Same contract as wsl_wgrad_tc2.
+// 3x3 weight gradient, v3 (filter columns in the MMA's M dimension).  Same contract as wsl_wgrad_tc; needs W % 8 == 0 and H % 16 == 0.
 WSL_API int wsl_wgrad_tc3(const void* src0, int C0, const void* src1, int C1, const void* dy, int CoutP, float* dw, int N, int H,
                           int W, int CoutReal, int ksize, int dtype, float* partial_ws, long long partial_floats, cudaStream_t stream) {
   WSL_REQUIRE(ksize == 3, "wsl_wgrad_tc3: 3x3 only");

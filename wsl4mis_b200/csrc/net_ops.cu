@@ -649,80 +649,22 @@ __device__ __forceinline__ DropCtx make_drop(float p, const uint8_t* mask, unsig
   return d;
 }
 
-// Statistics finalisation folded into the consumer (narrow layers, C <= 32): every block re-derives {scale, shift} from the convolution
-// epilogue's partial rows [nrows][2][C] (<= 296 x 64 floats, L2-resident) instead of waiting for a separate bn_finalize launch on the
-// forward critical path; block 0 also publishes save / ss / running statistics exactly like bn_finalize_kernel (same double sums, same
-// values up to the last bit of the double sums).
-struct BnFin {
-  const float* partials;   // null -> scale / shift are read from ss
-  int nrows;
-  long long P;
-  const float* gamma; const float* beta;
-  float* running_mean; float* running_var; long long* nbt;
-  float momentum, eps;
-  float* save; float* ss_out;
-};
-
 // A = dropout(leaky_relu(y*scale + shift)); optional fused 2x2 max-pool of A (DownBlock, unet.py:38).
 // PER_SAMPLE: ss holds {scale, shift} per image, [N][2][C] (per-sample BatchNorm, bn_stats_ps_kernel); reloaded when the pixel's image changes.
+// fp32 / fp16 storage: without a minimum-blocks hint ptxas fits the pooled path into 80 registers with a spill, and this kernel's
+// share of the fp16x3 step took 4 % longer (H100 80GB HBM3, 700 W power limit); with it, 95-112 registers and no spill.
+// bf16 (0: no hint) compiles to 64 registers without a spill.
 template <typename T, bool PER_SAMPLE = false>
-__global__ void __launch_bounds__(TPB) bn_act_fwd_kernel(
+__global__ void __launch_bounds__(TPB, std::is_same<T, __nv_bfloat16>::value ? 0 : 1) bn_act_fwd_kernel(
     const T* __restrict__ y, const float* __restrict__ ss, int N, int H, int W, int C, float slope,
     float drop_p, const uint8_t* __restrict__ mask, unsigned long long seed, const unsigned long long* seed_ptr,
-    T* __restrict__ act, T* __restrict__ pooled, uint8_t* __restrict__ pool_idx, const BnFin fin) {
+    T* __restrict__ act, T* __restrict__ pooled, uint8_t* __restrict__ pool_idx) {
   const int cg = C >> 3, rows = TPB / cg;
   const int g = threadIdx.x % cg, r = threadIdx.x / cg, c0 = g * 8;
   const DropCtx dc = make_drop(drop_p, mask, seed, seed_ptr);
   float sc[8], sh[8];
-  if (fin.partials != nullptr) {
-    __shared__ double s_sum[64];          // [2][C], C <= 32
-    __shared__ float s_ss[64];
-    // TPB / (2C) threads per statistic walk interleaved row subsets, then a fixed-order combine (as bn_finalize_kernel: 16 parts)
-    __shared__ double s_part[TPB];
-    const int nstat = 2 * C, parts = TPB / nstat;           // 8 (C = 16) or 4 (C = 32) threads per statistic
-    const int st = threadIdx.x % nstat, part = threadIdx.x / nstat;
-    double a = 0.0;
-    if (part < parts) {
-      const int which = st / C, c = st % C;
-      for (int bl = part; bl < fin.nrows; bl += parts) a += (double)__ldcg(&fin.partials[((size_t)bl * 2 + which) * C + c]);
-    }
-    s_part[threadIdx.x] = a;
-    __syncthreads();
-    if (threadIdx.x < nstat) {
-      double t = 0.0;
-      for (int q = 0; q < parts; ++q) t += s_part[q * nstat + threadIdx.x];
-      s_sum[threadIdx.x] = t;
-    }
-    __syncthreads();
-    if (threadIdx.x < C) {
-      const int c = threadIdx.x;
-      const double mean = s_sum[c] / (double)fin.P;
-      double var = s_sum[C + c] / (double)fin.P - mean * mean;
-      if (var < 0.0) var = 0.0;
-      const float invstd = (float)(1.0 / sqrt(var + (double)fin.eps));
-      const float scl = fin.gamma[c] * invstd, shf = fin.beta[c] - (float)mean * scl;
-      s_ss[c] = scl;
-      s_ss[C + c] = shf;
-      if (blockIdx.x == 0) {
-        fin.save[c] = (float)mean;
-        fin.save[C + c] = invstd;
-        fin.ss_out[c] = scl;
-        fin.ss_out[C + c] = shf;
-        if (fin.running_mean) {
-          fin.running_mean[c] = (1.f - fin.momentum) * fin.running_mean[c] + fin.momentum * (float)mean;
-          const double unb = (fin.P > 1) ? var * (double)fin.P / (double)(fin.P - 1) : var;
-          fin.running_var[c] = (1.f - fin.momentum) * fin.running_var[c] + fin.momentum * (float)unb;
-        }
-        if (c == 0 && fin.nbt) *fin.nbt += 1;
-      }
-    }
-    __syncthreads();
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { sc[j] = s_ss[c0 + j]; sh[j] = s_ss[C + c0 + j]; }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { sc[j] = ss[c0 + j]; sh[j] = ss[C + c0 + j]; }
-  }
+  for (int j = 0; j < 8; ++j) { sc[j] = ss[c0 + j]; sh[j] = ss[C + c0 + j]; }
   // loads are issued for all pixels of an iteration before the first use (the dropout branch would otherwise serialise them)
   int cur_n = 0;
   auto act8 = [&](int p, const float (&v)[8], float (&o)[8]) {
@@ -1603,38 +1545,16 @@ WSL_API int wsl_bn_eval_prepare(const float* gamma, const float* beta, const flo
   return wsl_check_launch("bn_eval_prepare");
 }
 
-static int bn_act_launch(const void* y, int dtype, const float* ss, int N, int H, int W, int C, float slope, float drop_p,
-                         const uint8_t* mask, unsigned long long seed, const unsigned long long* seed_ptr, void* act,
-                         void* pooled, uint8_t* pool_idx, const BnFin& fin, cudaStream_t stream) {
+WSL_API int wsl_bn_act_fwd(const void* y, int dtype, const float* ss, int N, int H, int W, int C, float slope, float drop_p,
+                           const uint8_t* mask, unsigned long long seed, const unsigned long long* seed_ptr, void* act,
+                           void* pooled, uint8_t* pool_idx, cudaStream_t stream) {
   WSL_REQUIRE(C % 8 == 0, "wsl_bn_act_fwd: C %% 8 != 0");
   WSL_REQUIRE(pooled == nullptr || (H % 2 == 0 && W % 2 == 0), "wsl_bn_act_fwd: pooling needs even H, W");
   WSL_REQUIRE(TPB % (C / 8) == 0 && (long long)N * H * W < (1LL << 31), "wsl_bn_act_fwd: unsupported C=%d or too many pixels", C);
   const long long items = (long long)N * H * W * (C / 8) / (pooled ? 4 : 1);
   WSL_DISPATCH_T(dtype, bn_act_fwd_kernel<T><<<grid_for((items + 1) / 2), TPB, 0, stream>>>(
-                            (const T*)y, ss, N, H, W, C, slope, drop_p, mask, seed, seed_ptr, (T*)act, (T*)pooled, pool_idx, fin));
+                            (const T*)y, ss, N, H, W, C, slope, drop_p, mask, seed, seed_ptr, (T*)act, (T*)pooled, pool_idx));
   return wsl_check_launch("bn_act_fwd");
-}
-
-WSL_API int wsl_bn_act_fwd(const void* y, int dtype, const float* ss, int N, int H, int W, int C, float slope, float drop_p,
-                           const uint8_t* mask, unsigned long long seed, const unsigned long long* seed_ptr, void* act,
-                           void* pooled, uint8_t* pool_idx, cudaStream_t stream) {
-  BnFin fin;
-  fin.partials = nullptr; fin.nrows = 0; fin.P = 0; fin.gamma = fin.beta = nullptr; fin.running_mean = fin.running_var = nullptr;
-  fin.nbt = nullptr; fin.momentum = 0.f; fin.eps = 0.f; fin.save = fin.ss_out = nullptr;
-  return bn_act_launch(y, dtype, ss, N, H, W, C, slope, drop_p, mask, seed, seed_ptr, act, pooled, pool_idx, fin, stream);
-}
-
-WSL_API int wsl_bn_finalize_act_fwd(const void* y, int dtype, const float* partials, int nrows, const float* gamma, const float* beta,
-                                    float* running_mean, float* running_var, long long* num_batches_tracked, float momentum, float eps,
-                                    float* save, float* ss, int N, int H, int W, int C, float slope, float drop_p, const uint8_t* mask,
-                                    unsigned long long seed, const unsigned long long* seed_ptr, void* act, void* pooled,
-                                    uint8_t* pool_idx, cudaStream_t stream) {
-  WSL_REQUIRE(C <= 32 && partials != nullptr && nrows >= 1, "wsl_bn_finalize_act_fwd: C <= 32 and partial rows are required (got C=%d)", C);
-  BnFin fin;
-  fin.partials = partials; fin.nrows = nrows; fin.P = (long long)N * H * W; fin.gamma = gamma; fin.beta = beta;
-  fin.running_mean = running_mean; fin.running_var = running_var; fin.nbt = num_batches_tracked; fin.momentum = momentum; fin.eps = eps;
-  fin.save = save; fin.ss_out = ss;
-  return bn_act_launch(y, dtype, ss, N, H, W, C, slope, drop_p, mask, seed, seed_ptr, act, pooled, pool_idx, fin, stream);
 }
 
 template <typename T>
@@ -1930,11 +1850,8 @@ WSL_API int wsl_bn_act_fwd_ps(const void* y, int dtype, const float* ss, int N, 
   WSL_REQUIRE(C % 8 == 0, "wsl_bn_act_fwd_ps: C %% 8 != 0");
   WSL_REQUIRE(pooled == nullptr || (H % 2 == 0 && W % 2 == 0), "wsl_bn_act_fwd_ps: pooling needs even H, W");
   WSL_REQUIRE(TPB % (C / 8) == 0 && (long long)N * H * W < (1LL << 31), "wsl_bn_act_fwd_ps: unsupported C=%d or too many pixels", C);
-  BnFin fin;
-  fin.partials = nullptr; fin.nrows = 0; fin.P = 0; fin.gamma = fin.beta = nullptr; fin.running_mean = fin.running_var = nullptr;
-  fin.nbt = nullptr; fin.momentum = 0.f; fin.eps = 0.f; fin.save = fin.ss_out = nullptr;
   const long long items = (long long)N * H * W * (C / 8) / (pooled ? 4 : 1);
   WSL_DISPATCH_T(dtype, (bn_act_fwd_kernel<T, true><<<grid_for((items + 1) / 2), TPB, 0, stream>>>(
-                            (const T*)y, ss, N, H, W, C, slope, drop_p, mask, seed, seed_ptr, (T*)act, (T*)pooled, pool_idx, fin)));
+                            (const T*)y, ss, N, H, W, C, slope, drop_p, mask, seed, seed_ptr, (T*)act, (T*)pooled, pool_idx)));
   return wsl_check_launch("bn_act_fwd_ps");
 }

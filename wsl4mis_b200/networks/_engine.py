@@ -120,13 +120,6 @@ class UNetExecutor:
         runs (optional): the decoder passes of one forward as (decoder index, feature transform) with transform in
         {None, "chan_drop", "feat_noise"} -- UNet_CCT_3H runs aux_decoder1 twice (unet.py:367-370) and never runs aux_decoder2."""
         assert precision in PRECISIONS
-        self.model = model
-        self.precision = precision
-        self.dt = PRECISIONS[precision]
-        self.act_dtype = {0: BF16, 1: torch.float32, 2: torch.float16}[self.dt]
-        self.split_tc = precision == "fp16x3"
-        # power-of-two factor carried by every activation gradient (set per backward from the batch shape; 1 = off)
-        self.scaled_grads = precision == "fp16"        # fp16x3 scales every staged operand by its own power of two instead
         if runs is None:
             runs = [(i, "chan_drop" if a else None) for i, a in enumerate(aux_dropout)]
         self.runs = list(runs)
@@ -176,11 +169,18 @@ class UNetExecutor:
             self.ds_heads.append(heads)
             built[didx] = (self.dec[-1], heads)
         self.n_class = decoders[0].out_conv.out_channels
-        self._init_runtime(model)
+        self._init_runtime(model, precision)
 
-    def _init_runtime(self, model):
-        """state shared by every planned network (the U-Net family here, PNet2D in _pnet_engine.py): parameter bookkeeping, buffers,
-        side streams, A/B switches"""
+    def _init_runtime(self, model, precision):
+        """state shared by every planned network (the U-Net family here, PNet2D in _pnet_engine.py): precision, parameter
+        bookkeeping, buffers, side streams"""
+        self.model = model
+        self.precision = precision
+        self.dt = PRECISIONS[precision]
+        self.act_dtype = {0: BF16, 1: torch.float32, 2: torch.float16}[self.dt]
+        self.split_tc = precision == "fp16x3"
+        # power-of-two factor carried by every activation gradient (set per backward from the batch shape; 1 = off)
+        self.scaled_grads = precision == "fp16"        # fp16x3 scales every staged operand by its own power of two instead
         self.params = [p for p in model.parameters()]
         used = set()
         for L in self.layers:
@@ -193,26 +193,15 @@ class UNetExecutor:
         self._bufs: Dict = {}
         self._live: List[int] = []
         self._seed_host = 0x5EED
-        self.use_tc = os.environ.get("WSL4MIS_NO_TC", "0") != "1"
-        self.use_tc_wgrad = os.environ.get("WSL4MIS_NO_TC_WGRAD", "0") != "1"
-        self.use_tc2 = os.environ.get("WSL4MIS_NO_TC2", "0") != "1"
-        self.wgrad_version = int(os.environ.get("WSL4MIS_WGRAD", "3"))
-        self.fuse_bn_stats = os.environ.get("WSL4MIS_NO_FUSED_STATS", "0") != "1"
-        self.defer_aux = os.environ.get("WSL4MIS_DEFER_AUX", "1") == "1"
-        self.fuse_first_bwd = os.environ.get("WSL4MIS_NO_FUSED_FIRST_BWD", "0") != "1"
-        self.deterministic_wgrad = os.environ.get("WSL4MIS_ATOMIC_WGRAD", "0") != "1"     # split-K partials + fixed-order finalize
-        # bn_finalize folded into bn_act_fwd for C <= 32 (every block re-derives scale / shift from the partial rows): measured SLOWER
-        # (12 launches 0.50 + 0.11 ms -> 0.91 ms: 1184 blocks each pay the fp64 prologue), so it stays off; kept for the A/B record
-        self.fold_finalize = os.environ.get("WSL4MIS_FOLDED_FINALIZE", "0") == "1"
+        self.use_tc = True               # False: every convolution on the CUDA-core direct kernels (a reference for the wgmma ones)
         self.on_decoders_done = None     # optional callback(gflat) between the decoder and encoder halves of backward()
         # Synchronised BatchNorm over data-parallel ranks (SURVEY 8(e)(2)): (world_size, process_group) or None.  Statistics of the
         # GLOBAL batch: forward all-reduces {sum, sum of squares} per layer, backward {sum dz, sum dz*xhat}; 2C floats each.
         self.sync_bn = None
-        self.multi_stream = os.environ.get("WSL4MIS_SINGLE_STREAM", "0") != "1"
+        self.multi_stream = True         # False: every launch on the current stream (per-kernel timing, single-chain networks)
         self._sides = {}                 # named side streams
         self._side_stack = []            # names of the side streams we are currently issuing on (innermost last)
         self._side_dirty = set()
-        self.bwd_streams = os.environ.get("WSL4MIS_BWD_STREAMS", "1") != "0"   # aux decoder backward chain on its own stream
         self._stat_bufs = {}
         self._stat_rows = ctypes.c_int(0)
         self._accumulate = False
@@ -325,7 +314,7 @@ class UNetExecutor:
 
     def _tc2_ok(self, layer_cin_list, H, W):
         """persistent / resident-weight / halo-view kernels: 8 x 16 pixel tiles"""
-        return (self.dt != 1 and self.use_tc and self.use_tc2 and all(c % 16 == 0 for c in layer_cin_list) and W % 8 == 0 and H % 16 == 0)
+        return (self.dt != 1 and self.use_tc and all(c % 16 == 0 for c in layer_cin_list) and W % 8 == 0 and H % 16 == 0)
 
     def _tc_ok(self, layer_cin_list, H, W):
         return (self.dt != 1 and self.use_tc and all(c % 16 == 0 for c in layer_cin_list) and W % 16 == 0 and H % 8 == 0)
@@ -346,9 +335,9 @@ class UNetExecutor:
         return t[0], t[1][1:]
 
     def conv_fwd(self, L: ConvLayer, srcs, out, out_mode, N, H, W, cout_store, src_f32=False, bn_out=None, srcC_override=None):
-        """bn_out = (save, ss) buffers: when the convolution runs on the persistent wgmma kernel the complete
+        """bn_out = (save, ss) buffers: when the convolution runs on conv_first or the persistent wgmma kernel the complete
         training-mode BatchNorm statistics of its output are produced by the kernel itself (partial rows in the epilogue,
-        finalised by the last CTA).  Returns True when that happened."""
+        finalised by bn_finalize).  Returns True when that happened."""
         pk = L.packs(self.dev)
         srcC = list(srcC_override) if srcC_override is not None else L.srcC     # (a materialised concat enters as ONE source)
         rows = False
@@ -364,18 +353,10 @@ class UNetExecutor:
         if not first:
             self.join_side("pack")        # packed operands are produced on a side stream at the start of forward()
         if first:
-            if bn_out is not None and self.fuse_bn_stats:
-                sb = self._stat_scratch()
-                bn = L.bn
-                call("wsl_conv_first", s0, L.conv.weight, L.conv.bias, out, self.dt, N, H, W, L.Cout, sb, ctypes.addressof(self._stat_rows))
-                self._untag()
-                if self.fold_finalize and L.Cout <= 32 and self.sync_bn is None:
-                    rows = (sb, self._stat_rows.value)          # finalised inside the consumer (bn_fwd)
-                else:
-                    self._finalize_stats(L, sb, self._stat_rows.value, N * H * W, bn_out[0], bn_out[1])
-                    rows = True
-            else:
-                call("wsl_conv_first", s0, L.conv.weight, L.conv.bias, out, self.dt, N, H, W, L.Cout, None, None)
+            rows = bn_out is not None
+            sb = self._stat_scratch() if rows else None
+            call("wsl_conv_first", s0, L.conv.weight, L.conv.bias, out, self.dt, N, H, W, L.Cout, sb,
+                 ctypes.addressof(self._stat_rows) if rows else None)
         elif not src_f32 and self._split_ok(srcC, H, W):
             st, inv = self._staged("x", srcs, srcC, N * H * W)
             call("wsl_conv_tc_split", st, L.Cin, inv, pk["f3"], pk["bias"], out, out_mode, N, H, W, L.CoutP, cout_store, L.ks, L.dil)
@@ -384,27 +365,19 @@ class UNetExecutor:
             call("wsl_conv_tc_dil", s0, c0, s1, c1, pk["bf"], pk["bias"], out, 0 if out_mode == 3 else out_mode, N, H, W, L.CoutP,
                  cout_store, L.ks, self.dt, L.dil)
         elif not src_f32 and self._tc2_ok(srcC, H, W):
-            if bn_out is not None and self.fuse_bn_stats and out_mode in (0, 3):
-                sb = self._stat_scratch()
-                bn = L.bn
-                call("wsl_conv_tc2", s0, c0, s1, c1, pk["bf"], pk["bias"], out, 0, N, H, W, L.CoutP, cout_store, L.ks, self.dt,
-                     sb, ctypes.addressof(self._stat_rows))
-                self._untag()                      # the finalize launch is not a convolution: keep it out of the conv roofline rows
-                if self.fold_finalize and L.Cout <= 32 and self.sync_bn is None:
-                    rows = (sb, self._stat_rows.value)          # finalised inside the consumer (bn_fwd)
-                else:
-                    self._finalize_stats(L, sb, self._stat_rows.value, N * H * W, bn_out[0], bn_out[1])
-                    rows = True
-            else:
-                call("wsl_conv_tc2", s0, c0, s1, c1, pk["bf"], pk["bias"], out, 0 if out_mode == 3 else out_mode, N, H, W, L.CoutP,
-                     cout_store, L.ks, self.dt, None, None)
+            rows = bn_out is not None and out_mode in (0, 3)
+            sb = self._stat_scratch() if rows else None
+            call("wsl_conv_tc2", s0, c0, s1, c1, pk["bf"], pk["bias"], out, 0 if out_mode == 3 else out_mode, N, H, W, L.CoutP,
+                 cout_store, L.ks, self.dt, sb, ctypes.addressof(self._stat_rows) if rows else None)
         elif not src_f32 and self._tc_ok(srcC, H, W):
             call("wsl_conv_tc", s0, c0, s1, c1, pk["bf"], pk["bias"], out, 0 if out_mode == 3 else out_mode, N, H, W, L.CoutP,
                  cout_store, L.ks, self.dt)
         else:
             call("wsl_conv_direct", s0, c0, s1, c1, f32, pk["wf"], pk["bias"], out, out_mode, N, H, W,
                  L.CinP, L.CoutP, cout_store, L.ks)
-        self._untag()
+        self._untag()                              # the finalize launch is not a convolution: keep it out of the conv roofline rows
+        if rows:
+            self._finalize_stats(L, sb, self._stat_rows.value, N * H * W, bn_out[0], bn_out[1])
         return rows
 
     def conv_dgrad(self, L: ConvLayer, i, dy, out, N, H, W):
@@ -434,9 +407,9 @@ class UNetExecutor:
         c0 = srcC[0]
         c1 = srcC[1] if len(srcC) > 1 else 0
         self._tag("wgrad", L, N, H, W, L.Cin, L.Cout)
-        tc = (not src_f32 and self.use_tc_wgrad and self._tc_ok(srcC, H, W)
-              and (L.CoutP < 128 or L.CoutP % 64 == 0))
-        split = (not src_f32 and self.use_tc_wgrad and self._split_ok(srcC, H, W) and (L.CoutP < 128 or L.CoutP % 64 == 0))
+        fits = L.CoutP <= 64 or L.CoutP % 64 == 0        # the dY boxes of wsl_wgrad_tc and wsl_wgrad_tc_split: one per 64 filters
+        tc = not src_f32 and self._tc_ok(srcC, H, W) and fits
+        split = not src_f32 and self._split_ok(srcC, H, W) and fits
         if src_f32 and L.Cin == 1 and L.Cout == 16 and L.ks == 3 and L.bn is not None:
             call("wsl_wgrad_first", s0, dy, self.dt, self.gview(L.conv.weight), N, H, W, L.Cout)
         elif split:
@@ -446,19 +419,15 @@ class UNetExecutor:
             tc = True
         elif L.dil != 1 and not src_f32:
             assert tc, "dilated weight gradient: per-tap wgmma kernel only"
-            pw = self._wgrad_partials() if self.deterministic_wgrad else None
+            pw = self._wgrad_partials()
             call("wsl_wgrad_tc_dil", s0, c0, s1, c1, dy, L.CoutP, self.gview(L.conv.weight), N, H, W, L.Cout, L.ks, self.dt, L.dil, pw,
-                 pw.numel() if pw is not None else 0)
-        elif tc and L.ks == 3 and self._tc2_ok(srcC, H, W) and self.wgrad_version == 3 and (L.CoutP <= 64 or L.CoutP % 128 == 0):
-            pw = self._wgrad_partials() if self.deterministic_wgrad else None
-            call("wsl_wgrad_tc3", s0, c0, s1, c1, dy, L.CoutP, self.gview(L.conv.weight), N, H, W, L.Cout, L.ks, self.dt, pw,
-                 pw.numel() if pw is not None else 0)
-        elif tc and L.ks == 3 and self._tc2_ok(srcC, H, W):
-            call("wsl_wgrad_tc2", s0, c0, s1, c1, dy, L.CoutP, self.gview(L.conv.weight), N, H, W, L.Cout, L.ks, self.dt)
+                 pw.numel())
+        elif tc and L.ks == 3 and self._tc2_ok(srcC, H, W) and (L.CoutP <= 64 or L.CoutP % 128 == 0):
+            pw = self._wgrad_partials()
+            call("wsl_wgrad_tc3", s0, c0, s1, c1, dy, L.CoutP, self.gview(L.conv.weight), N, H, W, L.Cout, L.ks, self.dt, pw, pw.numel())
         elif tc:
-            pw = self._wgrad_partials() if self.deterministic_wgrad else None
-            call("wsl_wgrad_tc", s0, c0, s1, c1, dy, L.CoutP, self.gview(L.conv.weight), N, H, W, L.Cout, L.ks, self.dt, pw,
-                 pw.numel() if pw is not None else 0)
+            pw = self._wgrad_partials()
+            call("wsl_wgrad_tc", s0, c0, s1, c1, dy, L.CoutP, self.gview(L.conv.weight), N, H, W, L.Cout, L.ks, self.dt, pw, pw.numel())
         else:
             call("wsl_wgrad_direct", s0, c0, s1, c1, 1 if (src_f32 or self.dt == 1) else self.dt, dy, self.dt, L.CoutP,
                  self.gview(L.conv.weight), self.gview(L.conv.bias) if L.bn is None else None, N, H, W, L.Cout, L.ks)
@@ -466,8 +435,7 @@ class UNetExecutor:
         # Bias gradient.  A conv bias that feeds training-mode BatchNorm has an exactly-zero gradient (BN removes the
         # per-channel mean); the reference holds ~1e-8 rounding noise there.  We leave the zero-filled bucket as is.
         if tc and L.bn is None:
-            call("wsl_channel_sum", dy, self.dt, N * H * W, L.CoutP, L.Cout, self.gview(L.conv.bias),
-                 self._ws("csum") if self.deterministic_wgrad else None)
+            call("wsl_channel_sum", dy, self.dt, N * H * W, L.CoutP, L.Cout, self.gview(L.conv.bias), self._ws("csum"))
 
     def bn_bufs(self, L, slot, tag):
         C = L.Cout
@@ -479,7 +447,6 @@ class UNetExecutor:
         pk = L.packs(self.dev)
         save = self.buf(slot, tag + ".save", (2 * C,), torch.float32)
         ss = self.buf(slot, tag + ".ss", (2 * C,), torch.float32)
-        deferred = stats_done if isinstance(stats_done, tuple) else None
         if training and self._bn_per_sample:
             # every image normalised by its own statistics (B batch-1 training forwards); {scale, shift} per image
             save = self.buf(slot, tag + ".save_ps", (N, 2 * C), torch.float32)
@@ -493,7 +460,7 @@ class UNetExecutor:
             self._untag()
             return save, ss
         if training and stats_done:
-            pass                       # save / ss come from the convolution epilogue's partial rows (bn_finalize, or folded in below)
+            pass                       # save / ss come from the convolution epilogue's partial rows (bn_finalize)
         elif training and self.sync_bn is not None:
             raw = self.buf(slot, tag + ".raw", (2 * C,), torch.float32)
             call("wsl_bn_stats", y, self.dt, N * H * W, C, bn.weight, bn.bias, None, None, None, float(bn.momentum), float(bn.eps),
@@ -511,13 +478,8 @@ class UNetExecutor:
         seed = self._layer_seed(L)
         esz = 4 if self.dt == 1 else 2
         self._tag_bytes("bn_act", L, N * H * W * C * esz * (2.25 if pooled is not None else 2.0))
-        if training and deferred is not None:
-            call("wsl_bn_finalize_act_fwd", y, self.dt, deferred[0], deferred[1], bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                 bn.num_batches_tracked, float(bn.momentum), float(bn.eps), save, ss, N, H, W, C, LRELU_SLOPE, p, mask, seed,
-                 self.seed_dev if mask is None and p > 0 else None, act, pooled, pool_idx)
-        else:
-            call("wsl_bn_act_fwd", y, self.dt, ss, N, H, W, C, LRELU_SLOPE, p, mask, seed, self.seed_dev if mask is None and p > 0 else None,
-                 act, pooled, pool_idx)
+        call("wsl_bn_act_fwd", y, self.dt, ss, N, H, W, C, LRELU_SLOPE, p, mask, seed, self.seed_dev if mask is None and p > 0 else None,
+             act, pooled, pool_idx)
         self._untag()
         return save, ss
 
@@ -740,7 +702,7 @@ class UNetExecutor:
             with self.on_side():                            # (a decoder that runs twice updates its running statistics twice)
                 drecs[di] = run_decoder(di, *self.dec[di])
         drecs[0] = run_decoder(0, *self.dec[0])
-        if not (defer_join and need_grad and self.defer_aux):
+        if not (defer_join and need_grad):
             self.join_side()           # otherwise backward() joins: the aux outputs must not be read before that
         rec["dec"] = drecs
         # deep-supervision outputs follow the decoders' main outputs: (dp1, dp2, dp3) = heads of up3, up2, up1 (unet.py:190)
@@ -793,7 +755,7 @@ class UNetExecutor:
                 self.conv_wgrad(l2, [r["a1"]], dy2, N, h, w)
             da1 = B(tag + ".da1", (N, h, w, C))
             self.conv_dgrad(l2, 0, dy2, da1, N, h, w)
-            if r["src_f32"] and l1.Cin == 1 and l1.Cout == 16 and l1.ks == 3 and self.fuse_first_bwd and self.sync_bn is None:
+            if r["src_f32"] and l1.Cin == 1 and l1.Cout == 16 and l1.ks == 3 and self.sync_bn is None:
                 # first layer: BatchNorm backward + weight gradient in one pass, dY never stored (no data gradient towards the image)
                 bn = l1.bn
                 self.last_backward_param_ids.update(id(q) for q in (bn.weight, bn.bias, l1.conv.weight, l1.conv.bias))
@@ -893,7 +855,7 @@ class UNetExecutor:
             # runs on the same stream as the first one, so the two never touch the shared gradient rows concurrently
             self._accumulate = base_accumulate or (didx in seen_decoders)
             seen_decoders.add(didx)
-            if di > 0 and self.bwd_streams and self.multi_stream:
+            if di > 0 and self.multi_stream:
                 nm = f"dec{didx}"
                 with self.on_side(nm):
                     decoder_bwd(di, ups, oc, g, rec["dec"][di])

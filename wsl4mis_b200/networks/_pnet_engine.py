@@ -11,18 +11,12 @@ fp16x3 (fp32-accurate split operands); there is no dilated CUDA-core kernel, so 
 import torch
 
 from .._lib import call
-from ._engine import ConvLayer, LRELU_SLOPE, UNetExecutor, PRECISIONS
+from ._engine import ConvLayer, LRELU_SLOPE, UNetExecutor
 
 
 class PNetExecutor(UNetExecutor):
     def __init__(self, model, precision="bf16"):
         assert precision in ("bf16", "fp16", "fp16x3"), "PNet2D runs in bf16, fp16 or fp16x3 mode (no dilated CUDA-core kernel)"
-        self.model = model
-        self.precision = precision
-        self.dt = PRECISIONS[precision]
-        self.act_dtype = {0: torch.bfloat16, 1: torch.float32, 2: torch.float16}[self.dt]
-        self.split_tc = precision == "fp16x3"
-        self.scaled_grads = precision == "fp16"
         self.in_chns, self.n_class, self.nf = model.in_chns, model.out_chns, model.num_filters
         nf = self.nf
         self.layers = []
@@ -38,7 +32,7 @@ class PNetExecutor(UNetExecutor):
         self.out1 = ConvLayer("out.conv1", model.out.conv1, None, 0.0, [2 * nf])
         self.out2 = ConvLayer("out.conv2", model.out.conv2, None, 0.0, [nf])
         self.layers += [self.cat1, self.cat2, self.out1, self.out2]
-        self._init_runtime(model)
+        self._init_runtime(model, precision)
         self.multi_stream = False           # a single chain: nothing to overlap
 
     def _lrelu(self, y, act, N, H, W, C):
