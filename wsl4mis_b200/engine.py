@@ -81,8 +81,8 @@ def _require_group(name, world_size, pg):
 
 
 def _aux_ids(model):
-    """ids of the aux decoder's parameters on a two-decoder model (unet_cct): steps that read main_seg only (SURVEY F7) skip them"""
-    return {id(q) for q in model.aux_decoder1.parameters()} if len(model.executor.dec) == 2 else set()
+    """ids of the parameters a step that reads main_seg only (SURVEY F7) skips: the aux decoder of unet_cct, none on the others"""
+    return set(model.executor.aux_param_ids)
 
 
 class _FlatSGDStep:
@@ -287,14 +287,16 @@ class TrainStep(_FlatSGDStep):
         if variant == "pce_variance":
             self.graph_enabled = False      # the ramp weight is a launch argument of the backward kernel
         self.beta = 0.5
-        self.two_heads = len(self.ex.dec) == 2
+        self.two_heads = self.ex.n_outputs == 2
         self.n_heads_trained = 2 if (variant == "dmpls") else 1
         if variant == "dmpls":
             assert self.two_heads, "dmpls needs a two-head model (unet_cct)"
-        # the encoder's parameters come first in parameters(): [0, enc_end) is final only at the very end of backward(), the
-        # decoder slice [enc_end, n_trained) ~2 ms earlier -- its all-reduce is issued from inside backward() on a side stream
-        self.enc_end = sum(q.numel() for q in model.encoder.parameters())
-        self.overlap_comm = self.world_size > 1 and os.environ.get("WSL4MIS_NO_COMM_OVERLAP", "0") != "1"
+        # U-Net: the encoder's parameters come first in parameters(): [0, enc_end) is final only at the very end of backward(), the
+        # decoder slice [enc_end, n_trained) ~2 ms earlier -- its all-reduce is issued from inside backward() on a side stream.
+        # An executor without that split (PNet2D: comm_split None) has its whole bucket all-reduced after backward().
+        self.enc_end = self.ex.comm_split
+        self.overlap_comm = (self.world_size > 1 and self.enc_end is not None
+                             and os.environ.get("WSL4MIS_NO_COMM_OVERLAP", "0") != "1")
         self.nccl_in_graph = os.environ.get("WSL4MIS_NCCL_IN_GRAPH", "0") == "1"     # opt-in: capture the collectives in the step graph
         if self.graph_enabled and not self.nccl_in_graph:
             self.overlap_comm = False        # a host-issued collective cannot sit inside the captured backward
@@ -590,7 +592,7 @@ class _TwoBatchStep(_FlatSGDStep):
         term, dl_u, extra = self._unsupervised(outs_u[0], teacher)
         loss = supervised + self.ramp_dev[0] * term
         self.parts = self._parts(ce, dice, supervised, term, extra)
-        rest = [None] * (len(ex.dec) - 1)
+        rest = [None] * (ex.n_outputs - 1)
         ex.backward(slot_u, [dl_u] + rest, zero_grads=True)
         return loss, ex.backward(slot_l, [dl_l] + rest, zero_grads=False)
 
@@ -736,7 +738,7 @@ class USTMStep(_FlatSGDStep):
         call("wsl_rot90", dr, B * C, H, (4 - k) % 4, 1, d)              # rotate the gradient back and add it to the pCE part
         loss = st[0] + self.ramp_dev[1] * cons
         self.parts = {"ce": st[0], "consistency": cons, "mask": mask}
-        g = ex.backward(slot, [d] + [None] * (len(ex.dec) - 1))
+        g = ex.backward(slot, [d] + [None] * (ex.n_outputs - 1))
         return loss, g
 
 
@@ -758,8 +760,8 @@ class S2LStep(TrainStep):
             raise NotImplementedError("global_batch semantics are not defined for the Scribble2Label step (run it with per-rank normalisers)")
         _require_group("S2LStep", world_size, kw.get("process_group"))
         ex = model.executor
-        if len(ex.dec) != 1 or any(ex.ds_heads) or not hasattr(ex, "enc_blocks"):
-            raise ValueError("Scribble2Label needs a single-output U-Net (train_s2l.py:228 takes softmax(model(img)))")
+        if ex.n_outputs != 1:
+            raise ValueError("Scribble2Label needs a single-output network (train_s2l.py:228 takes softmax(model(img)))")
         super().__init__(model, "pce", base_lr=base_lr, max_iterations=max_iterations, momentum=momentum, weight_decay=weight_decay,
                          graph=graph, world_size=world_size, **kw)
         self.thr_iter, self.thr_conf = int(thr_iter), float(thr_conf)
@@ -805,7 +807,8 @@ class S2LStep(TrainStep):
 
         Here `chunk` slices run as ONE per-sample-BatchNorm forward (exactly what `chunk` batch-1 training forwards compute, the
         running statistics updated in slice order across chunks); one kernel then does softmax at the back-zoom source pixel
-        and the EMA.  masks (tests): dropout keep masks {encoder block: uint8 [len(store), h, w, C]} for the whole pass.
+        and the EMA.  masks (tests): dropout keep masks for the whole pass, {encoder block: uint8 [len(store), h, w, C]} on the U-Net,
+        or PNet2D's two Dropout2d keep masks [uint8 [len(store), 128], uint8 [len(store), 64]].
 
         world_size > 1: rank r refreshes the contiguous slices `ddp.shard_range(len(store), r, world_size)` in chunks of its own,
         then each owner broadcasts its slices' contiguous range of the memory, so every rank ends with the whole memory (the next
@@ -824,8 +827,12 @@ class S2LStep(TrainStep):
             img = torch.empty(B, 1, size, size, dtype=torch.float32, device=dev)
             lab = torch.empty(B, size, size, dtype=torch.uint8, device=dev)
             call("wsl_augment_batch", store.images, store.labels, tab, B, size, size, img, lab)
-            mk = None if masks is None else {k: v[s: s + B] for k, v in masks.items()}
-            outs, _ = self.ex.forward(img, True, False, mk, None, bn_per_sample=True)
+            mk = ck = None
+            if isinstance(masks, dict):
+                mk = {k: v[s: s + B] for k, v in masks.items()}
+            elif masks is not None:
+                ck = [v[s: s + B] for v in masks]
+            outs, _ = self.ex.forward(img, True, False, mk, ck, bn_per_sample=True)
             max_hw = int(max(int(store.shapes[i, 0]) * int(store.shapes[i, 1]) for i in idx))
             call("wsl_s2l_refresh", outs[0], tab, B, size, max_hw, a, b, store.weight_live)
         if self.world_size > 1:
@@ -866,7 +873,7 @@ class DANStep(_TwoBatchStep):
                  betas=(0.9, 0.99), graph=True, world_size=1, process_group=None):
         _require_group("DANStep", world_size, process_group)
         ex = model.executor
-        if len(getattr(ex, "dec", ())) != 1 or any(getattr(ex, "ds_heads", ())):
+        if ex.n_outputs != 1:
             raise ValueError("DANStep needs a single-output segmentation network: the script takes torch.softmax(model(x), dim=1) "
                              "(train_deep_adversarial_network_2D.py:143-144), which fails on a tuple of outputs")
         super().__init__(model, base_lr, max_iterations, consistency, consistency_rampup, 0.9, 1e-4, graph, world_size, process_group)

@@ -170,6 +170,13 @@ class UNetExecutor:
             built[didx] = (self.dec[-1], heads)
         self.n_class = decoders[0].out_conv.out_channels
         self._init_runtime(model, precision)
+        # what the training steps (engine.py) read of an executor; PNetExecutor defines the same three
+        self.n_outputs = len(self.dec) + 3 * sum(1 for heads in self.ds_heads if heads)      # tensors forward() returns
+        # parameters a step that reads main_seg only leaves untrained (SURVEY F7): the aux decoder of unet_cct
+        self.aux_param_ids = {id(q) for q in model.aux_decoder1.parameters()} if len(self.dec) == 2 else set()
+        # the encoder's parameters come first in parameters(): a data-parallel step all-reduces the decoder slice of the bucket
+        # from inside backward() (on_decoders_done) and this prefix after it; None would turn that overlap off
+        self.comm_split = sum(q.numel() for q in encoder.parameters())
 
     def _init_runtime(self, model, precision):
         """state shared by every planned network (the U-Net family here, PNet2D in _pnet_engine.py): precision, parameter

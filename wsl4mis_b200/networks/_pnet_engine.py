@@ -7,6 +7,10 @@ dilated convolutions on the per-tap wgmma kernel (a tap is the TMA box at (y + d
 convolutions on the persistent resident-weight kernel, BatchNorm / LeakyReLU / channel dropout on the same elementwise kernels
 (LeakyReLU without BatchNorm: `wsl_lrelu_fwd` / `wsl_lrelu_bwd`).  Modes: bf16, fp16 and
 fp16x3 (fp32-accurate split operands); there is no dilated CUDA-core kernel, so the plain `fp32` cross-check mode is not offered.
+
+The training steps of engine.py run on it as on the U-Net executor: one output, no aux parameters, and no encoder/decoder split for
+a data-parallel step to overlap its all-reduce with (the whole bucket is reduced after backward).  Synchronised BatchNorm over
+data-parallel ranks (`sync_bn`, TrainStep(global_batch=True)) is not implemented for it.
 """
 import torch
 
@@ -34,6 +38,19 @@ class PNetExecutor(UNetExecutor):
         self.layers += [self.cat1, self.cat2, self.out1, self.out2]
         self._init_runtime(model, precision)
         self.multi_stream = False           # a single chain: nothing to overlap
+        self.n_outputs = 1
+        self.aux_param_ids = set()
+        self.comm_split = None              # no decoder half that finishes early: no all-reduce inside backward()
+
+    @property
+    def sync_bn(self):
+        return None
+
+    @sync_bn.setter
+    def sync_bn(self, value):
+        if value is not None:
+            raise NotImplementedError("synchronised BatchNorm (TrainStep(global_batch=True)) is not implemented for PNet2D; "
+                                      "its data-parallel steps keep per-rank BatchNorm statistics")
 
     def _lrelu(self, y, act, N, H, W, C):
         """nn.LeakyReLU between the 1x1 convolutions of ConcatBlock / OutPutBlock (pnet.py:60-61,94-95): no BatchNorm in front"""
@@ -53,7 +70,18 @@ class PNetExecutor(UNetExecutor):
         return d, cs
 
     # ---- forward ------------------------------------------------------------------------------------------------------------------
-    def forward(self, x, training, need_grad, masks=None, chan_keep=None, defer_join=False):
+    def forward(self, x, training, need_grad, masks=None, chan_keep=None, defer_join=False, bn_per_sample=False):
+        """x: fp32 [N, 1, H, W] CUDA -> ([fp32 NCHW logits], slot).  chan_keep: the two Dropout2d keep masks [N, 128] and [N, 64]
+        (None: drawn on the device).  bn_per_sample (training, no gradient): what N batch-1 training forwards compute -- every
+        BatchNorm normalises each image by its own statistics and the running statistics take the N updates in batch order;
+        Dropout2d stays on, one mask per image as in N separate forwards (the Scribble2Label refresh, train_s2l.py:221-228)."""
+        if bn_per_sample:
+            assert training and not need_grad, "bn_per_sample is a training-mode forward without gradient"
+            self._bn_per_sample = True
+            try:
+                return self.forward(x, training, need_grad, masks, chan_keep, defer_join)
+            finally:
+                self._bn_per_sample = False
         assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == self.in_chns == 1
         N, _, H, W = x.shape
         assert H % 8 == 0 and W % 16 == 0, "PNet2D on the wgmma kernels needs H % 8 == 0 and W % 16 == 0"
@@ -125,9 +153,12 @@ class PNetExecutor(UNetExecutor):
         self.last_backward_param_ids = set()
         B = lambda name, shape: self.buf(slot, "g." + name, shape)
         nvec = lambda C: N * H * W * C
-        g = grad_logits[0].contiguous()
-        dl = B("dl", (N, H, W, 16))
-        call("wsl_nchw_f32_to_nhwc", g, N, self.n_class, H, W, 16, dl, self.dt, S)
+        g = grad_logits[0]
+        if isinstance(g, tuple):                # ("nhwc16", tensor): already in the executor's layout and scaled by S
+            dl = g[1]
+        else:
+            dl = B("dl", (N, H, W, 16))
+            call("wsl_nchw_f32_to_nhwc", g.contiguous(), N, self.n_class, H, W, 16, dl, self.dt, S)
         # out.conv2 <- Dropout2d <- LeakyReLU <- out.conv1 <- Dropout2d <- LeakyReLU <- catblock.conv2 <- LeakyReLU <- catblock.conv1
         self.conv_wgrad(self.out2, [rec["d2"]], dl, N, H, W)
         dd2 = B("dd2", (N, H, W, nf))

@@ -9,7 +9,8 @@ line.  The loop is the scripts' skeleton (train_weakly_supervised_pCE_2D.py:56-1
 max_iterations // len(loader) + 1`` (the labelled loader for the semi-supervised scripts), validation every 200 iterations with
 best-model saves on a strict improvement, ``iter_{N}.pth`` every 3000, the stop at ``max_iterations``, and ``log.txt`` in the
 scripts' logging format under ``../model/{exp}_{fold}/{sup_type}``.  ``--precision`` (bf16 | fp16 | fp16x3 | fp32, default bf16)
-is the one flag the scripts lack; graph capture is always on.
+is the one flag the scripts lack; graph capture is always on.  ``--model pnet`` (PNet2D) runs every recipe but the two-output
+``..._pCE_ours_proposed.py``, in bf16, fp16 or fp16x3 (`check_model`).
 
 Several GPUs: ``torchrun --nproc_per_node W -m wsl4mis_b200.train train_X.py ARGS`` runs W ranks, batch-sharded data parallel
 with per-rank BatchNorm statistics and loss normalisers (DESIGN §7).  ``--batch_size`` stays the script's global batch: each rank
@@ -113,6 +114,7 @@ def _s2l_step(args, model, world_size=1):
                    graph=True, world_size=world_size)
 
 
+_DMPLS = _train_step("dmpls")
 _CE = (("info/loss_ce", _part("ce")),)
 _SEMI_COLS = (("info/loss_ce", _part("loss_ce", "parts")), ("info/loss_dice", _part("loss_dice", "parts")),
               ("info/consistency_loss", _part("consistency", "parts")))
@@ -133,7 +135,7 @@ RECIPES = {
         _flags(_WSS, (("consistency", float, 0.1), ("consistency_rampup", float, 200.0)), exp="ACDC_pCE_Inter&Intra_Class"),
         "single", _train_step("pce_variance"), _LOG2, _CE),
     "train_weakly_supervised_segmentation_pCE_ours_proposed.py": Recipe(
-        _flags(_WSS, exp="ACDC/pCE_SPS", model="unet_cct", max_iterations=60000, batch_size=6), "single", _train_step("dmpls"),
+        _flags(_WSS, exp="ACDC/pCE_SPS", model="unet_cct", max_iterations=60000, batch_size=6), "single", _DMPLS,
         'iteration %d : loss : %f, loss_ce: %f, loss_pse_sup: %f, alpha: %f', _CE + (("info/loss_pse_sup", _part("pse_sup")),),
         (("info/alpha", lambda step: step.beta),)),
     "train_fully_supervised_2D.py": Recipe(
@@ -190,7 +192,25 @@ def parse(argv):
     pre = argparse.ArgumentParser(add_help=False)
     pre.add_argument("--precision", choices=PRECISIONS, default="bf16")
     opts, rest = pre.parse_known_args(argv[1:])
-    return script, parser_for(script).parse_args(rest), opts.precision
+    args = parser_for(script).parse_args(rest)
+    check_model(script, args, opts.precision)
+    return script, args, opts.precision
+
+
+PNET_PRECISIONS = ("bf16", "fp16", "fp16x3")       # PNet2D's dilated convolutions have no CUDA-core (fp32 mode) kernel
+
+
+def check_model(script, args, precision):
+    """raise ValueError for the --model / --precision combinations no step runs, before any data or network is built:
+    PNet2D in fp32 mode, and PNet2D under the two-output recipe (pCE_ours_proposed unpacks ``outputs, outputs_aux1``)"""
+    if args.model != "pnet":
+        return
+    if precision not in PNET_PRECISIONS:
+        raise ValueError(f"--model pnet runs in {' / '.join(PNET_PRECISIONS)} (--precision {precision} is not available: PNet2D's "
+                         f"dilated convolutions run on the tensor-core kernels only)")
+    if recipe_for(script).step is _DMPLS:
+        raise ValueError(f"{os.path.basename(script)} needs a network with two outputs (--model unet_cct): it unpacks "
+                         f"'outputs, outputs_aux1 = model(volume_batch)', and PNet2D has one output")
 
 
 def rank_batch(script, batch_size, world_size):
@@ -377,6 +397,7 @@ def build(script, args, precision, rank=0, world_size=1):
     from .dataloaders.dataset import BaseDataSets, BaseDataSets_s2l, GpuLoader, S2LLoader, rank_streams
     from .networks.net_factory import net_factory
     recipe = recipe_for(script)
+    check_model(script, args, precision)
     bs = rank_batch(script, args.batch_size, world_size)
     random.seed(args.seed)
     np.random.seed(args.seed)
